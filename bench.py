@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of claxon_b200 (contract: see the task prompt / DESIGN.md §6).
+"""bench.py — headline benchmark of claxon_b200 (DESIGN.md §6).
 
 Metric (BASELINE.json): Msamples/s decoded, bit-exact, samples = sum(block_size * channels).
 Workload at N=1: BASELINE.json configs[1] ("c2"): batch of 1024 synthetic stereo 16-bit frames,
@@ -7,21 +7,19 @@ block size 4096, LPC order 8, Rice parameter 4, mid/side.  One *step* = one pass
 (`FrameReader::read_next_or_eof` for every frame of the batch) over one such batch ("unit").
 
   value  — kernel-only throughput, inputs resident in HBM.  The job is a list of units (128 distinct
-           batches per GPU: combined footprint 5 GB > L2, so no step finds its inputs or outputs in L2; 64 in
-           flight measured 528, 128 in flight 553 Gsamples/s on the same box); the list is
-           partitioned over the ranks by `claxon_b200.shard.plan_shards` (contiguous ranges balanced on
-           algorithmic bytes, no data-path collective: frames are independent, reference
-           src/frame.rs:603-605) and every rank cycles its units over `--streams` CUDA streams, i.e.
+           batches per GPU: combined footprint 5 GB, a hundred times the 50 MB L2 of an H100, so no step finds
+           its inputs or outputs in L2); the list is partitioned over the ranks by
+           `claxon_b200.shard.plan_shards` (contiguous ranges balanced on algorithmic bytes, no data-path
+           collective: frames are independent, reference src/frame.rs:603-605) and every rank cycles its units over `--streams` CUDA streams, i.e.
            many batches in flight: the steady-state regime of a decode service.  `--scaling weak`
            (default): `--inflight` units per rank; `--scaling strong`: a fixed corpus of `--units`
            units split over the ranks.  A lone 1024-frame batch is latency-bound by the serial LPC
            recurrence (SURVEY.md §7.3-3) and the sequential Rice walk; its figure is reported next to
-           it as `single_batch`.  A step takes ~15 us, so `--steps K` alone would be a sub-millisecond
-           window: the timed region is `repeats` x K steps issued back to back (no drain in between;
-           `repeats` is chosen so that the region holds >= --min-steps steps), it is measured
-           `--regions` times and the median region is reported; ms_per_step = region / (repeats * K).
-           Every batch's CUDA graph is instantiated when the batch is created and every batch is
-           decoded once before anything is timed, whatever --warmup says.
+           it as `single_batch`.  The timed region is exactly `--steps K` steps issued back to back (no
+           drain in between; per rank under weak scaling, split over the ranks under strong scaling);
+           ms_per_step = region / K.  Every batch's CUDA graph is instantiated when the batch is created,
+           and `--warmup W` untimed steps, at least one per batch, run before the region.
+           `--dump-outputs DIR` writes what the region's last step computed (dump_outputs()).
   e2e    — same metric through the public host-buffer call (`clx_decode_frames`): per step the
            compressed frames go pinned-host -> device and the full planar i32 PCM comes back.  The call
            is synchronous; `--e2e-callers` host threads (default 2, each with its own context and pinned
@@ -36,8 +34,8 @@ block size 4096, LPC order 8, Rice parameter 4, mid/side.  One *step* = one pass
   workloads — at N=1, short measurements of BASELINE.json's other configurations (c3, c4, c5) and of C2's
            independent-stereo variant by the same method, bit-exactness checked against the generator's PCM.
 
-`--impl reference` times that CPU port alone, same config/metric (the reference itself is Rust and
-cannot be built in this image or on the GPU box: no rustc / cargo on either).
+`--impl reference` times that CPU port alone, same config/metric (the reference itself is Rust; the
+benchmark does not build it).
 """
 from __future__ import annotations
 
@@ -134,17 +132,7 @@ def measured_peak_gbs():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def load_traffic():
-    """dram bytes per launch of the decode kernels from the committed ncu capture, if any."""
-    p = os.path.join(HERE, "profiles", "traffic.json")
-    try:
-        with open(p) as f:
-            return json.load(f)
-    except Exception:
-        return None
+        return 3350.0, "H100 SXM data sheet, 3.35 TB/s (not measured)"
 
 
 def cpu_model():
@@ -249,17 +237,6 @@ class Job:
                 return False
         return True
 
-    def steady(self, ctx, steps, streams, regions, sync=None):
-        """`regions` timed regions of `steps` steps each (round-robin over this rank's units); device ms each."""
-        n = len(self.batches)
-        ctx.run_steps(self.batches, max(n, 3), streams)  # every batch once, at least
-        out = []
-        for _ in range(max(1, regions)):
-            if sync:
-                sync()
-            out.append(ctx.run_steps(self.batches, steps, streams))
-        return out
-
     def per_steps(self, steps):
         """(samples, algorithmic bytes) that `steps` round-robin steps cover."""
         n = len(self.batches)
@@ -279,7 +256,8 @@ def short_line(cb, synth, ctx, workload, n_units, streams, min_ms=40.0):
     exact = job.exact(0)
     one = ctx.run_steps(job.batches, n_units, streams) / n_units  # ms per step, rough
     steps = max(n_units * 2, int(min_ms / max(one, 1e-3)))
-    ms = float(np.median(job.steady(ctx, steps, streams, 3)))
+    ctx.run_steps(job.batches, n_units, streams)  # every batch once
+    ms = float(np.median([ctx.run_steps(job.batches, steps, streams) for _ in range(3)]))
     samples, alg = job.per_steps(steps)
     peak, _ = measured_peak_gbs()
     cfg = unit_config(synth, workload, 0)
@@ -292,13 +270,37 @@ def short_line(cb, synth, ctx, workload, n_units, streams, min_ms=40.0):
     return line
 
 
+DUMP_BYTES = 64 * 1000 * 1000  # all arrays --dump-outputs writes, together
+
+
+def dump_outputs(out_dir, batch):
+    """Writes what the timed path computed for `batch` in its last step, as DeviceBatch.read() hands it to a caller:
+    per-frame `status` and bytes `consumed`, and `pcm`, the frames' planar samples one frame after the other (the
+    padding between frames left out).  Samples are float32 when they fit its 24-bit mantissa, else float64.  When they
+    exceed the size budget, a fixed seeded sample of them is written, with their positions in `pcm_index`."""
+    out, res = batch.read()
+    d = batch.descs
+    n = d["n_channels"].astype(np.int64) * d["block_size"].astype(np.int64)
+    pcm = np.concatenate([out[int(o):int(o) + int(k)] for o, k in zip(d["out_offset"], n)]) if d.size else out[:0]
+    arrays = {"status": res["status"].astype(np.float64), "consumed": res["consumed"].astype(np.float64)}
+    exact32 = pcm.size == 0 or int(np.abs(pcm.astype(np.int64)).max()) <= 1 << 24
+    pcm = pcm.astype(np.float32 if exact32 else np.float64)
+    room = DUMP_BYTES - sum(a.nbytes for a in arrays.values())
+    if pcm.nbytes > room:
+        idx = np.sort(np.random.default_rng(0).choice(pcm.size, size=room // (pcm.itemsize + 8), replace=False))
+        arrays["pcm_index"] = idx.astype(np.float64)
+        pcm = pcm[idx]
+    arrays["pcm"] = pcm
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=2000)
-    ap.add_argument("--min-steps", type=int, default=4000, help="the timed region holds at least this many steps (repeats x steps)")
-    ap.add_argument("--regions", type=int, default=3, help="timed regions; the median is reported")
-    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=4000, help="timed steps")
+    ap.add_argument("--warmup", type=int, default=5, help="untimed steps before them (at least one per batch)")
     ap.add_argument("--impl", default="claxon_b200", choices=["claxon_b200", "reference"])
     ap.add_argument("--workload", default="c2", choices=sorted(UNIT_FRAMES))
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"])
@@ -310,6 +312,8 @@ def main():
     ap.add_argument("--e2e-callers", type=int, default=2)
     ap.add_argument("--cpu-seconds", type=float, default=3.0)
     ap.add_argument("--no-extra", action="store_true", help="skip the short c3 / c4 / c5 lines at N=1")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output as DIR/<name>.npy (see dump_outputs)")
     args = ap.parse_args()
 
     rank, world, local = env_int("RANK", 0), env_int("WORLD_SIZE", 1), env_int("LOCAL_RANK", 0)
@@ -345,7 +349,7 @@ def main():
             "cpu_baseline": {"value": v, "unit": "Msamples/s", "cores": cores, "kind": "port", "cpu_model": cpu_model(),
                              "sample": f"{args.steps} x full {args.workload} batch ({batch.n_samples} samples)",
                              "note": "C restatement of claxon v0.4.3 (oracle/), frames sharded over threads; "
-                                     "claxon itself is Rust and cannot be built here (no rustc / cargo)"},
+                                     "claxon itself is Rust and is not built by the benchmark"},
             "e2e": {"value": v, "unit": "Msamples/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         }))
         return 0
@@ -413,7 +417,7 @@ def main():
     n_mine = hi - lo
     config.update({"parallelism": f"{n_units} units over {world} GPU(s) by plan_shards, no collective on the data path",
                    "units": n_units, "units_this_rank": n_mine, "streams": args.streams, "host": pin_note,
-                   "l2": f"steps cycle over {n_mine} distinct batches per GPU, footprint {job.alg_bytes / 1e6:.0f} MB > 126 MB L2"})
+                   "l2": f"steps cycle over {n_mine} distinct batches per GPU, footprint {job.alg_bytes / 1e6:.0f} MB > 50 MB L2"})
 
     exact = job.exact(0) if n_mine else True
 
@@ -429,33 +433,32 @@ def main():
             single.append(bt.kernel_ms())
         single_ms = float(np.median(single))
 
-    # ---- steady state
+    # ---- steady state: exactly --steps timed steps (weak: per rank; strong: a step = one unit of the corpus)
     if args.scaling == "weak":
-        repeats = max(1, -(-args.min_steps // max(1, args.steps)))
-        my_steps = repeats * args.steps        # per rank; the job's steps are world x that
+        my_steps = args.steps
         timed_steps = my_steps * world
-    else:  # a step = one unit of the corpus; a region = `repeats` passes over the whole corpus
-        repeats = max(1, -(-max(args.min_steps, args.steps) // n_units))
-        my_steps = repeats * n_mine
-        timed_steps = repeats * n_units
+    else:
+        my_steps = args.steps * hi // n_units - args.steps * lo // n_units
+        timed_steps = args.steps
+    if n_mine:
+        ctx.run_steps(job.batches, max(args.warmup, n_mine), args.streams)
+    barrier()
     sampler = ClockSampler(local)
     sampler.start()
     launches0 = ctx.launch_count
     t_wall0 = time.time()
-    regions = [max_over_ranks(r) for r in (job.steady(ctx, my_steps, args.streams, args.regions, barrier) if n_mine
-                                            else [0.0] * max(1, args.regions))]
+    ms = max_over_ranks(ctx.run_steps(job.batches, my_steps, args.streams) if n_mine and my_steps else 0.0)
     t_wall1 = time.time()
-    launches_all = ctx.launch_count - launches0
+    gpu_launches = ctx.launch_count - launches0
     barrier()
     clocks = sampler.stop(t_wall0, t_wall1)
-    ms = float(np.median(regions))
+    if args.dump_outputs and rank == 0 and n_mine and my_steps:
+        dump_outputs(args.dump_outputs, job.batches[(my_steps - 1) % n_mine])
     my_samples, my_alg = job.per_steps(my_steps) if n_mine else (0, 0)
-    gpu_launches = int(round(launches_all * my_steps / (my_steps * max(1, args.regions) + max(n_mine, 3)))) if n_mine else 0
     tot_samples, tot_alg = sum_over_ranks(my_samples), sum_over_ranks(my_alg)
     value = tot_samples / (ms / 1e3) / 1e6
     peak, peak_src = measured_peak_gbs()
     achieved = tot_alg / world / (ms / 1e3) / 1e9  # per GPU
-    traffic = load_traffic()
 
     # ---- end to end through the host-buffer call, pinned memory
     e2e = {}
@@ -555,8 +558,7 @@ def main():
             job.close()
             extra = {}
             # Mixed shapes keep fewer lanes of a warp busy, so these batches need more of them in flight than c2 to
-            # fill the chip (c4, 1100-frame units: 48 in flight 95, 96 -> 126, 128 -> 146 Gsamples/s,
-            # profiles/c4_units_in_flight_r02.txt); c5's frames are 128 times longer than their count suggests.
+            # fill the chip; c5's frames are 128 times longer than their count suggests.
             cx = cb.Context(device=local, n_streams=128, host_threads=host_threads)
             # (c2-indep: SURVEY §8d asks for the independent-stereo variant of C2 next to the mid/side headline)
             for wl, nu in (("c2-indep", 128), ("c3", 16), ("c4", 128), ("c5", 16)):
@@ -569,8 +571,8 @@ def main():
         e2e_main = e2e.get("e2e", {"value": None, "unit": "Msamples/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0})
         line = {
             "metric": METRIC, "value": value, "unit": "Msamples/s", "n_gpus": world, "steps": args.steps,
-            "warmup": max(args.warmup, 3), "ms_per_step": ms / timed_steps, "repeats": repeats, "timed_steps": timed_steps,
-            "region_ms": regions, "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None,
+            "warmup": args.warmup, "ms_per_step": ms / timed_steps, "timed_steps": timed_steps,
+            "region_ms": ms, "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None,
             "dtype": "int32 samples / int64 accumulate", "data": "synthetic", "config": config, "bit_exact": bool(exact),
             "clocks": clocks, "gpu_launches": gpu_launches,
             "single_batch": {"kernel_ms": single_ms, "value": (job.unit_samples[0] / (single_ms / 1e3) / 1e6) if single_ms else None,
@@ -578,10 +580,7 @@ def main():
             "e2e": e2e_main, "e2e_i16": e2e.get("e2e_i16"),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "peak_source": peak_src, "per": "GPU", "algorithmic_bytes_per_step": job.unit_alg[0] if n_mine else None,
-                         "kernels": "all kernels of a step's graph (index_frames_kernel + decode_subframes_kernel<0,false> do the work; "
-                                    "alone, same regime: 3.7 + 13.5 us of the step, profiles/SUMMARY_r02.md)",
-                         "traffic": (traffic or {}).get("dram_bytes_per_launch"),
-                         "traffic_source": (traffic or {}).get("source")},
+                         "kernels": "all kernels of a step's graph (index_frames_kernel + decode_subframes_kernel<0,false> do the work)"},
             "cpu_baseline": cpu, "host_demux": demux, "workloads": extra,
         }
         print(json.dumps(line))

@@ -1,4 +1,4 @@
-"""claxon_b200 — B200-native batched FLAC frame decoder behind claxon's API surface.
+"""claxon_b200 — H100-native batched FLAC frame decoder behind claxon's API surface.
 
 Host-side mirror of the reference interface for the per-frame decode path:
 

@@ -1,6 +1,6 @@
 """In-tree builds of the native pieces (no JIT cache: the .so files travel with the tree).
 
-* ``libclaxon_b200.so`` — the product: CUDA kernels for sm_100a + the C ABI of
+* ``libclaxon_b200.so`` — the product: CUDA kernels for sm_90a (H100) + the C ABI of
   ``include/claxon_b200.h`` + the C++ host side (demux, header parse, facade).
 * ``libclxsynth.so``    — the synthetic frame generator (plain C, host only).
 """
@@ -17,7 +17,7 @@ LIB = os.path.join(HERE, "libclaxon_b200.so")
 SYNTH = os.path.join(HERE, "libclxsynth.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-Wall", "-shared", "--use_fast_math", "-Xptxas", "-v",
 ]
 
@@ -49,7 +49,7 @@ def nvcc_path() -> str | None:
 
 
 def build_lib(force: bool = False, verbose: bool = False) -> str:
-    """Compiles the CUDA extension for sm_100a with nvcc (cross-compiles without a GPU).
+    """Compiles the CUDA extension for sm_90a with nvcc (cross-compiles without a GPU).
 
     CLX_EXPERIMENT=1 builds and selects ``libclaxon_b200_exp.so`` instead: the same sources with the
     measurement switches of tools/exp_*.py compiled in (-DCLX_EXPERIMENT); the product library has none."""
@@ -65,7 +65,7 @@ def build_lib(force: bool = False, verbose: bool = False) -> str:
     nvcc = nvcc_path()
     if nvcc is None:
         if os.path.exists(LIB):
-            return LIB  # GPU box without a toolchain: use the prebuilt library that travelled
+            return LIB  # a machine without the CUDA toolkit: use the library built elsewhere
         raise RuntimeError("nvcc not found and no prebuilt libclaxon_b200.so")
     extra = ["-DCLX_COOP_STATS"] if os.environ.get("CLX_COOP_STATS") else []
     if os.environ.get("CLX_EXPERIMENT"):

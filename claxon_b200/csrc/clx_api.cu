@@ -94,7 +94,7 @@ struct clx_ctx {
     std::vector<cudaStream_t> streams;
     std::string last_error;
     uint64_t launches = 0;
-    int sm_count = 148;
+    int sm_count = 132;  // H100 SXM; replaced by the device's own count in clx_ctx_create
     size_t smem_budget = 227 * 1024;
     bool use_coop = true;
     bool warp_per_frame = false;  // CLX_OPT_WARP_PER_FRAME: the warp-per-frame fast path (clx_coop.cu) everywhere
@@ -246,8 +246,7 @@ clx::CoopPlan make_plan(const clx_ctx* ctx, const clx_frame_desc* descs, size_t 
         max_bps = std::max<uint32_t>(max_bps, descs[i].bits_per_sample);
     }
     // (Frames with many channels and long blocks — BASELINE.json's stress shape, 8 x 16384 — are latency-bound on
-    // either fast path: the index lane walks (channels - 1) * block_size Rice codes alone.  Measured on 512 such
-    // frames: 13.0 ms through the lane-per-frame path, 16.8 ms through the warp-per-frame path; no special case.)
+    // either fast path: the index lane walks (channels - 1) * block_size Rice codes alone.  No special case.)
     if (clx::coop_plan(max_elems, max_ch, (uint32_t)n, ctx->sm_count, ctx->smem_budget, &plan) && !ctx->warp_per_frame &&
         !(latency_call && !ctx->lane_per_frame_always)) {
         plan.G = 2;

@@ -21,8 +21,9 @@
 //      block with 16-byte loads two trips ahead.  Wasted-bits shift (src/subframe.rs:216-225) and
 //      inter-channel decorrelation (src/frame.rs:319-389, partner channel = neighbouring lane, one
 //      shuffle) happen in registers; samples leave through a swizzled 32x32 shared-memory transpose
-//      as coalesced 16-byte stores, over the residuals they replace (the batch is launched back to
-//      back, so the residuals are normally still in the 126 MB L2 when they are read back).
+//      as coalesced 16-byte stores, over the residuals they replace (the two kernels run back to back,
+//      so when a batch's output fits the 50 MB L2 of an H100 — a 1024-frame C2 batch writes 34 MB —
+//      its residuals are read back from L2).
 //
 // Anything this path does not handle exactly — malformed input of any kind, the Rice escape code,
 // unary runs longer than a window, more than 8 channels — is not guessed at: the frame is flagged

@@ -1,4 +1,4 @@
-// clx_decode.cu — sm_100a frame-decode kernels of claxon_b200.
+// clx_decode.cu — sm_90a frame-decode kernels of claxon_b200.
 //
 // What runs here is everything claxon does between the frame-header parse and the
 // CRC-16 footer check of FrameReader::read_next_or_eof (reference src/frame.rs:701-742):

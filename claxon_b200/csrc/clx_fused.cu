@@ -134,11 +134,10 @@ struct DeviceIO {
 // Device IO policy of a lane, TMA flavour: a ring of two CHUNK-byte halves in shared memory, each filled by
 // one bulk copy (`cp.async.bulk`, SASS UBLKCP) that signals the half's own mbarrier
 // ---------------------------------------------------------------------------------
-// MEASUREMENT BUILD ONLY (-DCLX_RING_TMA, CLX_RING_TMA=1 in claxon_b200/_build.py): bit-exact (all GPU parity
-// tests pass with it) but 18 % slower than the cp.async ring above — a bulk copy takes uniform-register operands,
-// so the compiler serves 32 lanes with 32 sources through a loop of ~9 instructions per lane, against one LDGSTS
-// for the whole warp (profiles/ab_ring_tma_r02.json vs ab_ring_cpasync_r02.json).  Kept so that the comparison can
-// be repeated; the product library is built without it.
+// MEASUREMENT BUILD ONLY (-DCLX_RING_TMA, CLX_RING_TMA=1 in claxon_b200/_build.py): bit-exact, but a bulk copy
+// takes uniform-register operands, so the compiler serves 32 lanes with 32 sources through a loop of ~9
+// instructions per lane, against one LDGSTS for the whole warp with the cp.async ring above (DESIGN.md §3.1).
+// Kept so that the comparison can be made; the product library is built without it.
 // Chunk c of the frame (CHUNK bytes from its 16-byte aligned base) lives in half c & 1.  A half is re-armed
 // only after the cursor has left the chunk it held, so at most one copy per half is ever outstanding and the
 // parity to wait for simply alternates.  Reads past the end of the byte buffer see the buffer's last chunk
@@ -303,7 +302,7 @@ index_frames_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, const
 // Kernel 2: entropy decode + prediction + wasted shift + decorrelation, one lane per subframe
 // ---------------------------------------------------------------------------------
 #ifndef CLX_DEC_WARPS
-#define CLX_DEC_WARPS 2  // warps per decode CTA (1 and 4 were measured too: profiles/SUMMARY_r02.md)
+#define CLX_DEC_WARPS 2  // warps per decode CTA (CLX_DEC_WARPS=1 or 4 in claxon_b200/_build.py for comparison)
 #endif
 constexpr int DEC_WARPS = CLX_DEC_WARPS;
 constexpr uint32_t DEC_RQ = 8;
@@ -600,7 +599,9 @@ __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint
         };
         if (active) produce(rA, true);
         uint32_t t = head_end;
-        auto run = [&](auto mp) {
+        // Always inlined: left out of line (as nvcc does for sm_90a), every variable it captures by reference — the
+        // lane's bit window, the residual and sample registers — would live in local memory inside the loop.
+        auto run = [&](auto mp) __attribute__((always_inline)) {
             if (COMPACT) {
                 while (t + 8 < bulk_end) {
                     step(mp, rA, rB, t);

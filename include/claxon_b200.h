@@ -1,4 +1,4 @@
-/* claxon_b200.h — C ABI of the B200-native batched FLAC frame decoder.
+/* claxon_b200.h — C ABI of the H100-native batched FLAC frame decoder.
  *
  * This is the drop-in boundary for the per-frame decode path of ruuda/claxon
  * v0.4.3.  claxon has no FFI of its own; its boundary is the Rust API
@@ -12,7 +12,7 @@
  * ships raw frame bitstreams to the device, and everything below the header parse
  * and above the CRC-16 footer check — subframe::decode (src/subframe.rs:184-228),
  * decode_residual (:236-380), predict_fixed (:417-474), predict_lpc_* (:524-614),
- * decode_{left,right,mid}_side (src/frame.rs:319-389) — runs in sm_100a kernels.
+ * decode_{left,right,mid}_side (src/frame.rs:319-389) — runs in sm_90a kernels.
  *
  * Plain pointers and sizes only; no torch / C++ types cross this boundary.
  * There is NO CPU fallback: if no CUDA device is usable the create call fails

@@ -6,7 +6,7 @@
 //   claxon::Block::{time,len,duration,channels,channel,sample,into_buffer}  src/frame.rs:402-529
 //   claxon::Error {IoError, FormatError, Unsupported}      reference src/error.rs:18-45
 //
-// All decoding happens in libclaxon_b200.so (CUDA, sm_100a).  Nothing here decodes on the CPU.
+// All decoding happens in libclaxon_b200.so (CUDA, sm_90a).  Nothing here decodes on the CPU.
 #ifndef CLAXON_B200_HPP
 #define CLAXON_B200_HPP
 

@@ -1,10 +1,10 @@
 """Generates tests/golden/fixtures.npz from the reference's own test streams.
 
-Run in the authoring container (needs /root/reference; the GPU box does not have it):
+Run from the repository root with the path of a claxon v0.4.3 checkout (the tests never need it):
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <claxon checkout>
 
-For every stream under /root/reference/testsamples (incl. the fuzz corpus) it stores the raw
+For every stream under <claxon checkout>/testsamples (incl. the fuzz corpus) it stores the raw
 bytes, the status the oracle reports at open / first failing frame, and — for streams that
 decode — the oracle's planar PCM per frame, which is pinned independently by the STREAMINFO MD5
 (libFLAC's encoder-side digest) wherever the file carries one.  The npz is what the `-m gpu`
@@ -21,10 +21,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, ROOT)
 from oracle import oracle as O  # noqa: E402
 
-REF = "/root/reference/testsamples"
 
 
-def main():
+def main(ref_checkout):
+    REF = os.path.join(ref_checkout, "testsamples")
     out = {}
     names = []
     files = sorted(glob.glob(os.path.join(REF, "*.flac"))) + sorted(glob.glob(os.path.join(REF, "fuzz", "*.flac")))
@@ -77,4 +77,4 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])

@@ -1,7 +1,7 @@
 // ubench_pipes.cu — issue-rate microbenchmarks for the integer instructions the decode kernels lean on.
 // Each kernel runs 8 independent dependency chains per thread of one instruction kind; with 16 warps per SM
 // sub-partition the result is the pipe's throughput in warp-instructions per cycle per sub-partition.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/scratch/ubench_pipes tools/ubench_pipes.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/scratch/ubench_pipes tools/ubench_pipes.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -84,7 +84,8 @@ __global__ void k_lds(uint32_t* out, uint32_t seed, long long* cyc) {  // depend
 
 template <typename K>
 void run(const char* name, K kern, int threads, double ops_per_chain_step) {
-    int sms = 148;
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     uint32_t* out;
     long long* cyc;
     cudaMalloc(&out, sizeof(uint32_t) * sms * threads);
@@ -92,8 +93,8 @@ void run(const char* name, K kern, int threads, double ops_per_chain_step) {
     kern<<<sms, threads>>>(out, 12345u, cyc);
     kern<<<sms, threads>>>(out, 12345u, cyc);
     cudaDeviceSynchronize();
-    long long h[148];
-    cudaMemcpy(h, cyc, sizeof h, cudaMemcpyDeviceToHost);
+    long long h[1024];
+    cudaMemcpy(h, cyc, sizeof(long long) * sms, cudaMemcpyDeviceToHost);
     double avg = 0;
     for (int i = 0; i < sms; i++) avg += (double)h[i];
     avg /= sms;

@@ -21,7 +21,7 @@ import numpy as np
 from . import _lib
 from ._lib import (OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT)
 from ._lib import (FrameDesc, FrameResult, OPT_NO_VERIFY_CRC, OPT_GENERIC_KERNEL_ONLY, OPT_WARP_PER_FRAME, OPT_LANE_PER_FRAME,
-                   FRAME_VARIABLE_BLOCKING, FRAME_CRC16_VERIFIED,
+                   OPT_NO_GENERIC, OPT_NO_WIDE, FRAME_VARIABLE_BLOCKING, FRAME_CRC16_VERIFIED,
                    OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24)
 
 __all__ = ["Error", "Block", "FrameReader", "FlacReader", "FlacReaderOptions", "StreamInfo", "Context", "DeviceBatch",
@@ -197,14 +197,18 @@ class Context:
     """clx_ctx: one per host thread / GPU. Raises Error(NO_DEVICE) without a usable GPU."""
 
     def __init__(self, device: int = 0, verify_crc: bool = True, n_streams: int = 2, generic_only: bool = False,
-                 warp_per_frame: bool = False, lane_per_frame: bool = False, host_threads: int = 0):
+                 warp_per_frame: bool = False, lane_per_frame: bool = False, host_threads: int = 0,
+                 no_generic: bool = False, no_wide: bool = False):
         """Default: device-resident batches and large calls use the lane-per-frame index pass + lane-per-subframe
         decode pass (csrc/clx_fused.cu); small synchronous host-buffer calls (latency regime) use the
         warp-per-frame path (csrc/clx_coop.cu).  `warp_per_frame` / `lane_per_frame` force one of them everywhere,
-        `generic_only` bypasses both (testing, A/B measurements)."""
+        `generic_only` bypasses both (testing, A/B measurements).  `no_generic` / `no_wide` (testing) switch off
+        the kernels that take over what a fast path declined: such frames then come back with status -2 (the
+        generic kernel would have decoded them) or -3 (the lane-per-frame path's i64 second chance would have)."""
         self._L = _lib.load()
         flags = ((0 if verify_crc else OPT_NO_VERIFY_CRC) | (OPT_GENERIC_KERNEL_ONLY if generic_only else 0)
-                 | (OPT_WARP_PER_FRAME if warp_per_frame else 0) | (OPT_LANE_PER_FRAME if lane_per_frame else 0))
+                 | (OPT_WARP_PER_FRAME if warp_per_frame else 0) | (OPT_LANE_PER_FRAME if lane_per_frame else 0)
+                 | (OPT_NO_GENERIC if no_generic else 0) | (OPT_NO_WIDE if no_wide else 0))
         opts = _lib.Options(device, flags, n_streams, host_threads)
         h = C.c_void_p()
         _check(self._L.clx_ctx_create(C.byref(opts), C.byref(h)))

@@ -45,6 +45,8 @@ OPT_NO_VERIFY_CRC = 1
 OPT_GENERIC_KERNEL_ONLY = 2
 OPT_WARP_PER_FRAME = 4
 OPT_LANE_PER_FRAME = 8
+OPT_NO_GENERIC = 16
+OPT_NO_WIDE = 32
 OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT = 1, 2
 BATCH_BYTES_ON_DEVICE = 1
 OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24 = 0, 1, 2, 3

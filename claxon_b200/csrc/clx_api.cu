@@ -237,6 +237,8 @@ bool shape_order(const clx_frame_desc* descs, size_t lo, size_t hi, std::vector<
 constexpr size_t kLatencyRegimeFrames = 4096;
 clx::CoopPlan make_plan(const clx_ctx* ctx, const clx_frame_desc* descs, size_t n, bool latency_call = false) {
     clx::CoopPlan plan;
+    plan.no_generic = (ctx->flags & CLX_OPT_NO_GENERIC) != 0;
+    plan.no_wide = (ctx->flags & CLX_OPT_NO_WIDE) != 0;
     if (!ctx->use_coop) return plan;
     uint32_t max_elems = 0, max_ch = 0, max_bs = 0, max_bps = 0;
     for (size_t i = 0; i < n; i++) {

@@ -700,12 +700,11 @@ cudaError_t launch_decode(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_
     if (plan.G > 0 && d_params != nullptr) {
         e = launch_coop(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, d_generic, d_params, plan, stream);
         if (e != cudaSuccess) return e;
-#ifdef CLX_EXPERIMENT
-        if (g_exp_which & 8) return cudaGetLastError();  // measurement only: leave the fast path's verdicts as they are
-#endif
+        // index pass + two decode instances (+ two WIDE ones) / entropy + prediction
+        if (launches) *launches += plan.G == 2 ? (plan.no_wide ? 3 : 5) : 2;
+        if (plan.no_generic) return cudaGetLastError();  // testing: leave the fast path's verdicts as they are
         decode_frames_kernel<12><<<grid, block, 0, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results,
                                                              d_need_hi, d_generic, CLX_INTERNAL_NEED_GENERIC);
-        if (launches) *launches += plan.G == 2 ? 5 : 2;  // index pass + four decode instances / entropy + prediction
     } else {
         decode_frames_kernel<12><<<grid, block, 0, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results,
                                                              d_need_hi, nullptr, 0);

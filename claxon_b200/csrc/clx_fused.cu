@@ -824,7 +824,8 @@ cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_fra
         const size_t dyn = 0;
 #endif
 #define CLX_DEC(C, W) decode_subframes_kernel<C, W><<<g2, b2, dyn, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, params, CH, ch_log2, n_pwarps, d_need_generic, d_need_generic + 2)
-        CLX_DEC(0, false); CLX_DEC(1, false); CLX_DEC(0, true); CLX_DEC(1, true);
+        CLX_DEC(0, false); CLX_DEC(1, false);
+        if (!plan.no_wide) { CLX_DEC(0, true); CLX_DEC(1, true); }
 #undef CLX_DEC
     }
     return cudaGetLastError();

@@ -10,8 +10,10 @@
 #define CLX_INTERNAL_NEED_HIGH_ORDER (-1)
 // Device-only marker: the cooperative kernel declined the frame (anything irregular: malformed
 // input, escape codes, oversize frames ...); the generic lane-per-frame kernel decodes it.
+// Returned through the C ABI only under CLX_OPT_NO_GENERIC (the generic kernel then does not run).
 #define CLX_INTERNAL_NEED_GENERIC (-2)
 // Device-only marker of the throughput path: decode the frame again with the i64 accumulator (clx_fused.cu).
+// Returned through the C ABI only under CLX_OPT_NO_WIDE (the second chance then does not run).
 #define CLX_INTERNAL_NEED_WIDE (-3)
 
 namespace clx {
@@ -21,6 +23,8 @@ struct CoopPlan {          // whether / how a batch uses the fast path
     uint32_t channels = 0;      // channel slots per frame (power of two >= max channels in the batch)
     size_t smem_bytes = 0;
     uint32_t max_bs = 0;        // G == 2: largest block size in the batch
+    bool no_generic = false;    // CLX_OPT_NO_GENERIC: no generic-kernel launch after a fast path
+    bool no_wide = false;       // CLX_OPT_NO_WIDE: G == 2 without its i64 second chance
 };
 // clx_fused.cu: `which` bit 0 = index pass, bit 1 = decode pass (both in the product; single ones in measurement builds)
 size_t seq_scratch_bytes(const CoopPlan& plan, uint32_t n_frames);
@@ -50,7 +54,7 @@ uint32_t output_elem_size(uint32_t mode);
 cudaError_t launch_interleave(const clx_frame_desc* d_descs, uint32_t n_frames, uint32_t max_frame_elems, const int32_t* d_planar,
                               void* d_dst, uint32_t mode, cudaStream_t stream);
 #ifdef CLX_EXPERIMENT
-extern int g_exp_which;  // measurement builds only: bit 0 = index pass, bit 1 = decode pass
+extern int g_exp_which;  // measurement builds only: bit 0 = index pass, bit 1 = decode pass of G == 2
 extern int g_exp_dyn_smem;
 #endif
 

@@ -85,6 +85,12 @@ typedef struct clx_options {
 #define CLX_OPT_GENERIC_KERNEL_ONLY 2u /* testing: bypass the fast path */
 #define CLX_OPT_WARP_PER_FRAME 4u      /* the warp-per-frame fast path everywhere (default: only for small synchronous calls) */
 #define CLX_OPT_LANE_PER_FRAME 8u      /* the lane-per-frame fast path everywhere, also for small synchronous calls */
+/* Testing: a fast path's verdicts are left as they are.  NO_GENERIC: the generic kernel does not re-decode the frames
+ * a fast path declined (a call without a fast path still runs it); such a frame comes back with status -2.
+ * NO_WIDE: the lane-per-frame path skips its i64 second chance; a frame that needed it comes back with status -3.
+ * Neither status ever reaches the caller without these options. */
+#define CLX_OPT_NO_GENERIC 16u
+#define CLX_OPT_NO_WIDE 32u
 
 typedef struct clx_ctx clx_ctx;     /* one per host thread / GPU; owns device scratch */
 typedef struct clx_batch clx_batch; /* a device-resident batch (bytes + descriptors + output) */

@@ -17,6 +17,10 @@
 extern "C" {
 #endif
 
+/* Two negative values appear only under the test options of claxon_b200.h, which switch off the kernels
+ * that would otherwise take a frame over: -2 (CLX_OPT_NO_GENERIC: a fast path declined the frame, the generic
+ * kernel would have decoded it) and -3 (CLX_OPT_NO_WIDE: the frame needed the lane-per-frame path's i64 second
+ * chance).  No other call ever returns a negative status. */
 typedef enum clx_status {
     CLX_OK = 0,
     /* Ok(None): end of stream while reading the first two header bytes

@@ -241,9 +241,7 @@ class Context:
             ends = descs["out_offset"] + descs["n_channels"].astype(np.uint64) * descs["block_size"]
             out_elems = int(ends.max()) if descs.size else 0
         if out is None:
-            n = max(1, out_elems)
-            out = (np.empty(n, dtype=np.int16) if mode == OUT_INTERLEAVED_I16 else
-                   np.empty(3 * n, dtype=np.uint8) if mode == OUT_INTERLEAVED_I24 else np.empty(n, dtype=np.int32))
+            out = _out_array(out_elems, mode)
         results = np.zeros(descs.size, dtype=RESULT_DTYPE)
         _check(self._L.clx_decode_frames_to(self._h, buf.ctypes.data, buf.size, descs.ctypes.data, descs.size,
                                             out.ctypes.data, max(1, out_elems), results.ctypes.data, mode), self)
@@ -272,33 +270,44 @@ class Context:
     def host_free(self, arr: np.ndarray):
         self._L.clx_host_free(arr.ctypes.data)
 
-    def upload(self, data, descs: np.ndarray, out_elems: int) -> "DeviceBatch":
-        return DeviceBatch(self, data, descs, out_elems)
+    def upload(self, data, descs: np.ndarray, out_elems: int, mode: int = OUT_PLANAR_I32) -> "DeviceBatch":
+        """A device-resident batch.  `mode`: the form its output is kept in, as for decode_frames (out_offset and
+        out_elems count samples in every mode)."""
+        return DeviceBatch(self, data, descs, out_elems, mode=mode)
 
-    def adopt(self, device_ptr: int, nbytes: int, descs: np.ndarray, out_elems: int) -> "DeviceBatch":
+    def adopt(self, device_ptr: int, nbytes: int, descs: np.ndarray, out_elems: int,
+              mode: int = OUT_PLANAR_I32) -> "DeviceBatch":
         """A batch whose frame bytes already sit in this GPU's memory at `device_ptr` (e.g. a torch tensor's
         data_ptr() after the NCCL scatter of claxon_b200.shard.scatter_batch): copied device to device."""
-        return DeviceBatch(self, None, descs, out_elems, device_ptr=device_ptr, nbytes=nbytes)
+        return DeviceBatch(self, None, descs, out_elems, device_ptr=device_ptr, nbytes=nbytes, mode=mode)
+
+
+def _out_array(out_elems: int, mode: int) -> np.ndarray:
+    """A host array for `out_elems` samples in output mode `mode`: int16, 3 bytes per sample as uint8, or int32."""
+    n = max(1, out_elems)
+    return (np.empty(n, dtype=np.int16) if mode == OUT_INTERLEAVED_I16 else
+            np.empty(3 * n, dtype=np.uint8) if mode == OUT_INTERLEAVED_I24 else np.empty(n, dtype=np.int32))
 
 
 class DeviceBatch:
     """clx_batch: frames resident in HBM; decode() launches the kernels only."""
 
     def __init__(self, ctx: Context, data, descs: np.ndarray, out_elems: int, device_ptr: int | None = None,
-                 nbytes: int = 0):
+                 nbytes: int = 0, mode: int = OUT_PLANAR_I32):
         self.ctx = ctx
         self.descs = np.ascontiguousarray(descs, dtype=DESC_DTYPE)
         self.out_elems = int(out_elems)
+        self.mode = int(mode)
         h = C.c_void_p()
         if device_ptr is None:
             buf = _as_u8(data)
             self.nbytes = int(buf.size)
-            _check(ctx._L.clx_batch_create(ctx._h, buf.ctypes.data, buf.size, self.descs.ctypes.data,
-                                           self.descs.size, self.out_elems, C.byref(h)), ctx)
+            _check(ctx._L.clx_batch_create_to(ctx._h, buf.ctypes.data, buf.size, self.descs.ctypes.data, self.descs.size,
+                                              self.out_elems, 0, self.mode, C.byref(h)), ctx)
         else:
             self.nbytes = int(nbytes)
-            _check(ctx._L.clx_batch_create_ex(ctx._h, device_ptr, self.nbytes, self.descs.ctypes.data, self.descs.size,
-                                              self.out_elems, _lib.BATCH_BYTES_ON_DEVICE, C.byref(h)), ctx)
+            _check(ctx._L.clx_batch_create_to(ctx._h, device_ptr, self.nbytes, self.descs.ctypes.data, self.descs.size,
+                                              self.out_elems, _lib.BATCH_BYTES_ON_DEVICE, self.mode, C.byref(h)), ctx)
         self._h = h
 
     def decode(self, stream: int = 0):
@@ -313,10 +322,11 @@ class DeviceBatch:
         return float(ms.value)
 
     def read(self):
-        out = np.empty(max(1, self.out_elems), dtype=np.int32)
+        """Returns (out, results); `out` is in the batch's mode: int32, int16, or uint8 with 3 bytes per sample."""
+        out = _out_array(self.out_elems, self.mode)
         results = np.zeros(self.descs.size, dtype=RESULT_DTYPE)
-        _check(self.ctx._L.clx_batch_read(self.ctx._h, self._h, out.ctypes.data, out.size,
-                                          results.ctypes.data), self.ctx)
+        _check(self.ctx._L.clx_batch_read_to(self.ctx._h, self._h, out.ctypes.data, max(1, self.out_elems),
+                                             results.ctypes.data), self.ctx)
         return out, results
 
     @property

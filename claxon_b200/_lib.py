@@ -79,9 +79,11 @@ SYMBOLS = {
     "clx_decode_frames_to": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _vp, _sz, _vp, C.c_uint32]),
     "clx_batch_create": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _sz, C.POINTER(_vp)]),
     "clx_batch_create_ex": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _sz, C.c_uint32, C.POINTER(_vp)]),
+    "clx_batch_create_to": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _sz, C.c_uint32, C.c_uint32, C.POINTER(_vp)]),
     "clx_batch_decode": (C.c_int, [_vp, _vp, C.c_uint32]),
     "clx_batch_sync": (C.c_int, [_vp, _vp]),
     "clx_batch_read": (C.c_int, [_vp, _vp, _vp, _sz, _vp]),
+    "clx_batch_read_to": (C.c_int, [_vp, _vp, _vp, _sz, _vp]),
     "clx_batch_destroy": (None, [_vp, _vp]),
     "clx_batch_device_out": (_vp, [_vp]),
     "clx_batch_device_bytes": (_vp, [_vp]),

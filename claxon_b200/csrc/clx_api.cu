@@ -142,6 +142,13 @@ struct clx_batch {
     std::vector<uint32_t> h_len;
     std::vector<uint32_t> order;   // device position -> caller's frame index (empty: identity), see shape_order()
     bool device_crc = false;       // bytes came from device memory: the CRC-16 check runs on the device, inside the graph
+    // Output mode (CLX_OUT_*).  Interleaved batches hand out d_conv; d_out stays their planar scratch.  The lane-per-frame
+    // path writes I32 / I16 into d_conv itself (clx::FusedOut; d_mark: the frames the generic kernel took over); every
+    // other path, and I24, decodes to d_out and converts all frames inside the graph (launch_interleave).
+    uint32_t mode = CLX_OUT_PLANAR_I32;
+    void* d_conv = nullptr;
+    uint8_t* d_mark = nullptr;
+    uint32_t max_frame_elems = 0;
 };
 
 namespace {
@@ -196,6 +203,14 @@ void precompute_crc(clx_ctx* ctx, const uint8_t* bytes, const clx_frame_desc* de
 }
 
 void build_graph(clx_ctx* ctx, clx_batch* b);
+
+// The interleaved modes hold a sample in 2 / 3 bytes only for frames of at most 16 / 24 bits per sample.
+bool frames_fit_mode(const clx_frame_desc* descs, size_t n_frames, uint32_t mode) {
+    const uint32_t max_bps = mode == CLX_OUT_INTERLEAVED_I16 ? 16u : mode == CLX_OUT_INTERLEAVED_I24 ? 24u : 32u;
+    for (size_t i = 0; i < n_frames; i++)
+        if (descs[i].bits_per_sample > max_bps) return false;
+    return true;
+}
 
 // Everything the kernels assume about a caller-supplied descriptor (the C ABI does not trust it).
 bool valid_desc(const clx_frame_desc& d, size_t nbytes, size_t out_elems) {
@@ -329,9 +344,7 @@ int clx_decode_frames_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, cons
     if (n_frames == 0) return CLX_OK;
     uint8_t* const out = static_cast<uint8_t*>(out_v);
     const size_t esize = clx::output_elem_size(mode);
-    const uint32_t max_bps = mode == CLX_OUT_INTERLEAVED_I16 ? 16u : mode == CLX_OUT_INTERLEAVED_I24 ? 24u : 32u;
-    for (size_t i = 0; i < n_frames; i++)
-        if (descs[i].bits_per_sample > max_bps) return CLX_ERR_INVALID_ARGUMENT;
+    if (!frames_fit_mode(descs, n_frames, mode)) return CLX_ERR_INVALID_ARGUMENT;
     CU(ctx, cudaSetDevice(ctx->device));
     if (!out) return CLX_ERR_INVALID_ARGUMENT;
     for (size_t i = 0; i < n_frames; i++)
@@ -463,9 +476,16 @@ int clx_batch_create(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const cl
 
 int clx_batch_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
                         size_t out_elems, uint32_t batch_flags, clx_batch** out) {
-    if (!ctx || !out || (!bytes && nbytes) || (!descs && n_frames)) return CLX_ERR_INVALID_ARGUMENT;
+    return clx_batch_create_to(ctx, bytes, nbytes, descs, n_frames, out_elems, batch_flags, CLX_OUT_PLANAR_I32, out);
+}
+
+int clx_batch_create_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
+                        size_t out_elems, uint32_t batch_flags, uint32_t mode, clx_batch** out) {
+    if (!ctx || !out || (!bytes && nbytes) || (!descs && n_frames) || mode > CLX_OUT_INTERLEAVED_I24)
+        return CLX_ERR_INVALID_ARGUMENT;
     const bool on_device = (batch_flags & CLX_BATCH_BYTES_ON_DEVICE) != 0;
     *out = nullptr;
+    if (!frames_fit_mode(descs, n_frames, mode)) return CLX_ERR_INVALID_ARGUMENT;
     CU(ctx, cudaSetDevice(ctx->device));
     for (size_t i = 0; i < n_frames; i++)
         if (!valid_desc(descs[i], nbytes, out_elems)) return CLX_ERR_INVALID_ARGUMENT;
@@ -475,6 +495,9 @@ int clx_batch_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const
     b->out_elems = out_elems;
     b->n_frames = (uint32_t)n_frames;
     b->plan = make_plan(ctx, descs, n_frames);
+    b->mode = mode;
+    for (size_t i = 0; i < n_frames; i++)
+        b->max_frame_elems = std::max<uint32_t>(b->max_frame_elems, (uint32_t)descs[i].n_channels * descs[i].block_size);
     cudaError_t e = cudaMalloc((void**)&b->d_bytes, b->buf_bytes);
     if (e == cudaSuccess) e = cudaMemset(b->d_bytes, 0, b->buf_bytes);
     if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_descs, std::max<size_t>(1, n_frames) * sizeof(clx_frame_desc));
@@ -482,6 +505,8 @@ int clx_batch_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const
     if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_results, std::max<size_t>(1, n_frames) * sizeof(clx_frame_result));
     if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_need_hi, 4 * sizeof(int));
     if (e == cudaSuccess) e = cudaMalloc(&b->d_params, clx::coop_params_bytes(b->plan, b->n_frames) + 16);
+    if (e == cudaSuccess && mode != CLX_OUT_PLANAR_I32) e = cudaMalloc(&b->d_conv, (out_elems + 8) * clx::output_elem_size(mode));
+    if (e == cudaSuccess && mode != CLX_OUT_PLANAR_I32) e = cudaMalloc((void**)&b->d_mark, std::max<size_t>(1, n_frames));
     if (e == cudaSuccess) e = cudaMemcpy(b->d_bytes, bytes, nbytes, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
         if (shape_order(descs, 0, n_frames, b->order)) {
@@ -514,6 +539,24 @@ int clx_batch_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const
 }  // extern "C"
 
 namespace {
+// The launch sequence of one decode of a batch: the decode kernels, the device CRC-16 (bytes from device memory),
+// and the conversion to the batch's interleaved mode where the decode pass does not write that mode itself.
+cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
+    const bool fused = (b->mode == CLX_OUT_INTERLEAVED_I32 || b->mode == CLX_OUT_INTERLEAVED_I16) && b->plan.G == 2;
+    const clx::FusedOut fo{b->mode, b->d_conv, b->d_mark, b->max_frame_elems};
+    cudaError_t e = clx::launch_decode(b->d_bytes, b->buf_bytes, b->d_descs, b->n_frames, b->d_out, b->d_results, b->d_need_hi,
+                                       b->d_params, b->plan, st, launches, fused ? &fo : nullptr);
+    if (e == cudaSuccess && b->device_crc) {
+        e = clx::launch_crc16(b->d_bytes, b->d_descs, b->n_frames, b->d_results, st);
+        (*launches)++;
+    }
+    if (e == cudaSuccess && b->mode != CLX_OUT_PLANAR_I32 && !fused) {
+        e = clx::launch_interleave(b->d_descs, b->n_frames, b->max_frame_elems, b->d_out, b->d_conv, b->mode, st);
+        (*launches)++;
+    }
+    return e;
+}
+
 // Captures the batch's launch sequence once; called from clx_batch_create so that no decode ever pays for
 // (or is timed with) a graph instantiation.
 void build_graph(clx_ctx* ctx, clx_batch* b) {
@@ -526,9 +569,7 @@ void build_graph(clx_ctx* ctx, clx_batch* b) {
     uint64_t n = 0;
     cudaError_t e = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
     if (e == cudaSuccess) {
-        cudaError_t e1 = clx::launch_decode(b->d_bytes, b->buf_bytes, b->d_descs, b->n_frames, b->d_out, b->d_results,
-                                            b->d_need_hi, b->d_params, b->plan, st, &n);
-        if (e1 == cudaSuccess && b->device_crc) { e1 = clx::launch_crc16(b->d_bytes, b->d_descs, b->n_frames, b->d_results, st); n++; }
+        cudaError_t e1 = launch_batch(b, st, &n);
         e = cudaStreamEndCapture(st, &g);
         if (e1 != cudaSuccess) e = e1;
     }
@@ -549,9 +590,7 @@ int enqueue_batch(clx_ctx* ctx, clx_batch* b, cudaStream_t st) {
     }
     // No graph: two decodes of one batch share its flag words and parameter records, so they must not overlap.
     if (b->ev_idle) CU(ctx, cudaStreamWaitEvent(st, b->ev_idle, 0));
-    CU(ctx, clx::launch_decode(b->d_bytes, b->buf_bytes, b->d_descs, b->n_frames, b->d_out, b->d_results, b->d_need_hi,
-                               b->d_params, b->plan, st, &ctx->launches));
-    if (b->device_crc) { CU(ctx, clx::launch_crc16(b->d_bytes, b->d_descs, b->n_frames, b->d_results, st)); ctx->launches++; }
+    CU(ctx, launch_batch(b, st, &ctx->launches));
     if (!b->ev_idle) CU(ctx, cudaEventCreateWithFlags(&b->ev_idle, cudaEventDisableTiming));
     CU(ctx, cudaEventRecord(b->ev_idle, st));
     return CLX_OK;
@@ -584,11 +623,11 @@ int clx_batch_last_kernel_ms(clx_ctx* ctx, clx_batch* b, float* ms) {
     return CLX_OK;
 }
 
-int clx_batch_read(clx_ctx* ctx, clx_batch* b, int32_t* out, size_t out_elems, clx_frame_result* results) {
-    if (!ctx || !b) return CLX_ERR_INVALID_ARGUMENT;
-    int rc = clx_batch_sync(ctx, b);
-    if (rc) return rc;
-    if (out) CU(ctx, cudaMemcpy(out, b->d_out, std::min(out_elems, b->out_elems) * sizeof(int32_t), cudaMemcpyDeviceToHost));
+}  // extern "C"
+
+namespace {
+// Per-frame results of the batch's last decode at the caller's frame indices, with the host-side CRC-16 verdicts.
+int read_results(clx_ctx* ctx, clx_batch* b, clx_frame_result* results) {
     if (results) {
         if (b->order.empty()) {
             CU(ctx, cudaMemcpy(results, b->d_results, b->n_frames * sizeof(clx_frame_result), cudaMemcpyDeviceToHost));
@@ -619,12 +658,31 @@ int clx_batch_read(clx_ctx* ctx, clx_batch* b, int32_t* out, size_t out_elems, c
     }
     return CLX_OK;
 }
+}  // namespace
+
+extern "C" {
+
+int clx_batch_read(clx_ctx* ctx, clx_batch* b, int32_t* out, size_t out_elems, clx_frame_result* results) {
+    if (!ctx || !b || b->mode != CLX_OUT_PLANAR_I32) return CLX_ERR_INVALID_ARGUMENT;
+    return clx_batch_read_to(ctx, b, out, out_elems, results);
+}
+
+int clx_batch_read_to(clx_ctx* ctx, clx_batch* b, void* out, size_t out_elems, clx_frame_result* results) {
+    if (!ctx || !b) return CLX_ERR_INVALID_ARGUMENT;
+    int rc = clx_batch_sync(ctx, b);
+    if (rc) return rc;
+    if (out)
+        CU(ctx, cudaMemcpy(out, clx_batch_device_out(b), std::min(out_elems, b->out_elems) * clx::output_elem_size(b->mode),
+                           cudaMemcpyDeviceToHost));
+    return read_results(ctx, b, results);
+}
 
 void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
     (void)ctx;
     if (!b) return;
     cudaFree(b->d_bytes); cudaFree(b->d_descs); cudaFree(b->d_out); cudaFree(b->d_results); cudaFree(b->d_need_hi);
     cudaFree(b->d_params);
+    cudaFree(b->d_conv); cudaFree(b->d_mark);
     if (b->graph) cudaGraphExecDestroy(b->graph);
     if (b->ev_idle) cudaEventDestroy(b->ev_idle);
     if (b->ev_start) cudaEventDestroy(b->ev_start);
@@ -674,7 +732,7 @@ int clx_ctx_run_steps(clx_ctx* ctx, clx_batch** batches, size_t n_batches, uint3
     return rc;
 }
 
-void* clx_batch_device_out(clx_batch* b) { return b ? b->d_out : nullptr; }
+void* clx_batch_device_out(clx_batch* b) { return b ? (b->mode == CLX_OUT_PLANAR_I32 ? (void*)b->d_out : b->d_conv) : nullptr; }
 void* clx_batch_device_bytes(clx_batch* b) { return b ? b->d_bytes : nullptr; }
 
 // Pinned host memory for callers that want true asynchronous copies.

@@ -768,9 +768,9 @@ size_t coop_params_bytes(const CoopPlan& plan, uint32_t n_frames) {
 
 cudaError_t launch_coop(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
                         int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, void* d_params,
-                        const CoopPlan& plan, cudaStream_t stream) {
+                        const CoopPlan& plan, cudaStream_t stream, uint32_t mode) {
     if (plan.G == 2)
-        return launch_seq(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, d_need_generic, d_params, plan, stream, 3);
+        return launch_seq(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, d_need_generic, d_params, plan, stream, 3, mode);
     SubParams* params = reinterpret_cast<SubParams*>(d_params);
     const uint32_t CH = plan.channels;
     dim3 g1((n_frames + ENT_WARPS - 1) / ENT_WARPS), b1(ENT_WARPS * 32);

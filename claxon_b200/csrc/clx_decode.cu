@@ -689,7 +689,8 @@ decode_frames_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes,
 // ---------------------------------------------------------------------------------
 cudaError_t launch_decode(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs,
                           uint32_t n_frames, int32_t* d_out, clx_frame_result* d_results, int* d_flags,
-                          void* d_params, const CoopPlan& plan, cudaStream_t stream, uint64_t* launches) {
+                          void* d_params, const CoopPlan& plan, cudaStream_t stream, uint64_t* launches,
+                          const FusedOut* fused) {
     if (n_frames == 0) return cudaSuccess;
     const uint32_t per_cta = WARPS_PER_CTA * 32;
     dim3 grid((n_frames + per_cta - 1) / per_cta), block(per_cta);
@@ -698,11 +699,18 @@ cudaError_t launch_decode(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_
     cudaError_t e = cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream);  // [0] generic, [1] 32 taps, [2] i64 retry
     if (e != cudaSuccess) return e;
     if (plan.G > 0 && d_params != nullptr) {
-        e = launch_coop(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, d_generic, d_params, plan, stream);
+        if (fused) e = launch_coop(d_bytes, buf_bytes, d_descs, n_frames, static_cast<int32_t*>(fused->d_dst), d_results, d_generic,
+                                   d_params, plan, stream, fused->mode);
+        else e = launch_coop(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, d_generic, d_params, plan, stream);
         if (e != cudaSuccess) return e;
         // index pass + two decode instances (+ two WIDE ones) / entropy + prediction
         if (launches) *launches += plan.G == 2 ? (plan.no_wide ? 3 : 5) : 2;
         if (plan.no_generic) return cudaGetLastError();  // testing: leave the fast path's verdicts as they are
+        if (fused) {  // the frames the generic kernel is about to take over, whatever the fast path wrote for them
+            e = launch_mark_status(d_results, n_frames, CLX_INTERNAL_NEED_GENERIC, fused->d_mark, d_generic, stream);
+            if (e != cudaSuccess) return e;
+            if (launches) *launches += 1;
+        }
         decode_frames_kernel<12><<<grid, block, 0, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results,
                                                              d_need_hi, d_generic, CLX_INTERNAL_NEED_GENERIC);
     } else {
@@ -714,6 +722,14 @@ cudaError_t launch_decode(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_
     decode_frames_kernel<32><<<grid, block, 0, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results,
                                                          d_need_hi, d_need_hi, CLX_INTERNAL_NEED_HIGH_ORDER);
     if (launches) *launches += 2;
+    if (fused) {
+        // The marked frames' planar samples -> interleaved, over every element of each: nothing the fast path wrote
+        // for them survives.  Gated like the 12-tap instance: exits at once when the fast path declined nothing.
+        e = launch_interleave(d_descs, n_frames, fused->max_frame_elems, d_out, fused->d_dst, fused->mode, stream, fused->d_mark,
+                              d_generic);
+        if (e != cudaSuccess) return e;
+        if (launches) *launches += 1;
+    }
     return cudaGetLastError();
 }
 

@@ -16,7 +16,8 @@
 //      Samples leave through a swizzled 32x32 shared-memory transpose; the flush handles the two channels
 //      of a frame together, which turns the wasted-bits shift (src/subframe.rs:216-225) and the
 //      inter-channel decorrelation (src/frame.rs:319-389) into a few operations per PAIR of 16-byte
-//      vectors, and writes planar i32 as whole 128-byte lines.
+//      vectors, and writes planar i32 as whole 128-byte lines — or, for a device-resident batch in an
+//      interleaved i32 / i16 mode, the interleaved samples themselves (DESIGN.md §3.1).
 //
 // HBM traffic per frame: its bytes once for the decode, the bytes of all channels but the last once more
 // for the index pass, 224 bytes of parameters per subframe, and the planar i32 output once.
@@ -343,12 +344,48 @@ __device__ __forceinline__ void seq_trip(int32_t (&v)[TAPS + U], const int32_t (
 // are neighbouring channels of one frame when the batch has at least two channel slots — `ca` on the even
 // row is then the frame's stereo mode if the pair is its (channel 0, channel 1) — and two unrelated mono
 // frames otherwise.
+// Output mode OM (a template parameter of the decode pass, CLX_OUT_* values): CLX_OUT_PLANAR_I32 writes claxon's
+// Block layout; CLX_OUT_INTERLEAVED_I32 / _I16 write element t * nch + c of the frame (sample t of channel c) as a
+// little-endian integer of 4 / 2 bytes.  In the interleaved instances `out` is the FRAME's first element (the same
+// for all its rows), bit 0 of `meta` says that this address is 16-byte aligned, and bits 24-27 / 28-31 hold the
+// frame's channel count and the row's channel.
 struct __align__(16) SeqRow {
     int32_t* out;   // subframe's first output element (nullptr: idle row)
     uint32_t bs;    // block size
     uint32_t meta;  // bit 0: 16-byte stores allowed; bits 8-15: wasted bits; bits 16-19 (even rows): 8 left/side,
                     // 9 side/right, 10 mid/side, 0 independent
 };
+
+// ---- interleaved output ----
+template <int OM>
+__device__ __forceinline__ void il_store(uint8_t* frame, uint32_t e, int32_t v) {
+    if (OM == CLX_OUT_INTERLEAVED_I16) reinterpret_cast<int16_t*>(frame)[e] = (int16_t)v;  // `sample as i16`
+    else reinterpret_cast<int32_t*>(frame)[e] = v;
+}
+// Four samples of a stereo frame's two channels (steps g .. g+3) as four interleaved (left, right) pairs at element
+// 2g: one 16-byte store for i16, two for i32.  `p` is that element's address, 16-byte aligned.
+template <int OM>
+__device__ __forceinline__ void il_store_pairs(uint8_t* p, const int4& a, const int4& b) {
+    if (OM == CLX_OUT_INTERLEAVED_I16) {
+        *reinterpret_cast<uint4*>(p) = make_uint4(__byte_perm(a.x, b.x, 0x5410), __byte_perm(a.y, b.y, 0x5410),
+                                                  __byte_perm(a.z, b.z, 0x5410), __byte_perm(a.w, b.w, 0x5410));
+    } else {
+        reinterpret_cast<int4*>(p)[0] = make_int4(a.x, b.x, a.y, b.y);
+        reinterpret_cast<int4*>(p)[1] = make_int4(a.z, b.z, a.w, b.w);
+    }
+}
+// Steps g .. g+3 of one row, element by element (any frame base, any channel count; steps past the block are skipped).
+template <int OM>
+__device__ __forceinline__ void il_store_row(const SeqRow& r, uint32_t g, const int4& v) {
+    if (r.out == nullptr || g >= r.bs) return;
+    uint8_t* frame = reinterpret_cast<uint8_t*>(r.out);
+    const uint32_t nch = (r.meta >> 24) & 15u, c = r.meta >> 28;
+    const uint32_t e = g * nch + c;
+    il_store<OM>(frame, e, v.x);
+    if (g + 1 < r.bs) il_store<OM>(frame, e + nch, v.y);
+    if (g + 2 < r.bs) il_store<OM>(frame, e + 2 * nch, v.z);
+    if (g + 3 < r.bs) il_store<OM>(frame, e + 3 * nch, v.w);
+}
 
 __device__ __forceinline__ uint32_t seq_tile_word(uint32_t row, uint32_t col) {
     return row * 32 + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3));
@@ -382,7 +419,10 @@ __device__ __forceinline__ void mid_side(int32_t& a, int32_t& b) {
 // 16-byte vectors of a row pair (rows 2p, 2p+1), so each store instruction of the warp covers four whole
 // 128-byte lines — scattering the lanes over more rows costs the load/store unit a wavefront per line.
 // CHECKED = false is for tiles wholly inside every active row with 16-byte stores allowed everywhere.
-template <bool CHECKED>
+// Interleaved (OM != planar): a quarter holds whole frames (CH <= 8 channel slots, a frame's channels are CH
+// consecutive rows), and a lane writes what it holds: four interleaved pairs when its rows are a stereo frame's two
+// channels and the frame base is 16-byte aligned, else element by element.
+template <bool CHECKED, int OM = CLX_OUT_PLANAR_I32>
 __device__ __forceinline__ void seq_flush_quarter(const int32_t* tile, const SeqRow* rows, uint32_t g0, uint32_t q, uint32_t lane,
                                                   bool any_wasted) {
     const uint32_t grp = lane & 7;
@@ -402,7 +442,16 @@ __device__ __forceinline__ void seq_flush_quarter(const int32_t* tile, const Seq
         a.x = (int32_t)((uint32_t)a.x + (uint32_t)b.x); a.y = (int32_t)((uint32_t)a.y + (uint32_t)b.y);
         a.z = (int32_t)((uint32_t)a.z + (uint32_t)b.z); a.w = (int32_t)((uint32_t)a.w + (uint32_t)b.w);
     }
-    if (CHECKED) {
+    if constexpr (OM != CLX_OUT_PLANAR_I32) {
+        // (an idle row's meta has no channel count: never a pair)
+        const bool pair = ((i0.meta >> 24) & 15u) == 2 && (i0.meta >> 28) == 0;
+        if (pair && (!CHECKED || ((i0.meta & 1u) != 0 && g + 4 <= i0.bs))) {
+            il_store_pairs<OM>(reinterpret_cast<uint8_t*>(i0.out) + 2 * g * (OM == CLX_OUT_INTERLEAVED_I16 ? 2 : 4), a, b);
+        } else {  // unaligned frame bases (packed or odd out_offset), the end of a block, frames of 1 or 3..8 channels
+            il_store_row<OM>(i0, g, a);
+            il_store_row<OM>(i1, g, b);
+        }
+    } else if (CHECKED) {
         seq_store_vec(i0.out, i0.bs, (i0.meta & 1u) != 0, g, a);
         seq_store_vec(i1.out, i1.bs, (i1.meta & 1u) != 0, g, b);
     } else {
@@ -410,11 +459,11 @@ __device__ __forceinline__ void seq_flush_quarter(const int32_t* tile, const Seq
         if (i1.out != nullptr) *reinterpret_cast<int4*>(i1.out + g) = b;
     }
 }
-template <bool CHECKED>
+template <bool CHECKED, int OM = CLX_OUT_PLANAR_I32>
 __device__ __forceinline__ void seq_flush(const int32_t* tile, const SeqRow* rows, uint32_t g0, uint32_t lane, bool any_wasted) {
     __syncwarp();
 #pragma unroll
-    for (uint32_t i = 0; i < 4; i++) seq_flush_quarter<CHECKED>(tile, rows, g0, i, lane, any_wasted);
+    for (uint32_t i = 0; i < 4; i++) seq_flush_quarter<CHECKED, OM>(tile, rows, g0, i, lane, any_wasted);
     __syncwarp();
 }
 
@@ -433,7 +482,9 @@ __device__ __forceinline__ void sts128(uint32_t addr, int32_t a, int32_t b, int3
 // inside every row.
 //   tile_s: shared address of the tile to write out;  outp_s: shared address of the warp's 32 row pointers;
 //   lc0 / lc1: the lane's constant offsets into the tile for rows (2p, 2p+1) of its quarter (see decode_rows).
-template <int UCA>
+// Interleaved (OM != planar, only for batches of stereo frames: CH == 2): rows (2p, 2p+1) are one frame's left and
+// right channel, and the lane's four samples of each are four interleaved pairs at the frame's element 2g.
+template <int UCA, int OM = CLX_OUT_PLANAR_I32>
 __device__ __forceinline__ void flush_quarter_fast(uint32_t tile_s, uint32_t outp_s, uint32_t g0, uint32_t quarter, uint32_t lane,
                                                    uint32_t lc0, uint32_t lc1) {
     const uint32_t a0 = tile_s + quarter * 1024u + lc0;
@@ -448,8 +499,14 @@ __device__ __forceinline__ void flush_quarter_fast(uint32_t tile_s, uint32_t out
         ob = make_int4(a.x - hx, a.y - hy, a.z - hz, a.w - hw);
     }
     const uint32_t off = (g0 + (lane & 7u) * 4u) * 4u;  // bytes
-    *reinterpret_cast<int4*>(p0 + off) = oa;
-    *reinterpret_cast<int4*>(p1 + off) = ob;
+    if constexpr (OM == CLX_OUT_INTERLEAVED_I16) {
+        il_store_pairs<OM>(reinterpret_cast<uint8_t*>(p0) + off, oa, ob);  // element 2g, 2 bytes each: byte 4g
+    } else if constexpr (OM == CLX_OUT_INTERLEAVED_I32) {
+        il_store_pairs<OM>(reinterpret_cast<uint8_t*>(p0) + 2 * off, oa, ob);
+    } else {
+        *reinterpret_cast<int4*>(p0 + off) = oa;
+        *reinterpret_cast<int4*>(p1 + off) = ob;
+    }
 }
 
 // The body of a subframe lane: residuals from the lane's own Rice decoder, recurrence, tile, flush.
@@ -457,7 +514,7 @@ __device__ __forceinline__ void flush_quarter_fast(uint32_t tile_s, uint32_t out
 // end), so the 32x32 tile fills row by row in step and is flushed as whole lines.
 //   tile_s: shared address of the warp's two tiles (8 KB, 8 KB-aligned: the other tile is `addr ^ 4096`).
 //   FMODE: 0 = general flush; 1 / 2 = flush_quarter_fast applies, without stereo decorrelation / mid-side.
-template <int TAPS, int U, typename ACC, int FMODE>
+template <int TAPS, int U, typename ACC, int FMODE, int OM>
 __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint32_t order, uint32_t shift,
                                             const SeqParams* __restrict__ sp, bool active, int32_t* tile, uint32_t tile_s,
                                             const SeqRow* pr, uint32_t outp_s, uint32_t lane, bool all_vec,
@@ -505,7 +562,7 @@ __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint
             h[0] = val;
             int32_t* fill = tile_ptr(fill_s);
             fill[seq_tile_word(lane, t & 31)] = val;
-            if ((t & 31) == 31) seq_flush<true>(fill, pr, t - 31, lane, any_wasted);
+            if ((t & 31) == 31) seq_flush<true, OM>(fill, pr, t - 31, lane, any_wasted);
         }
     };
     guarded(0, head_end);
@@ -563,9 +620,9 @@ __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint
         auto after = [&](uint32_t t) {
             if (have_drain) {  // a tile inside [head_end, bulk_end) lies inside every active row
                 const uint32_t g0 = (t & ~31u) - 32, quarter = (t >> 3) & 3;
-                if (FMODE != 0) flush_quarter_fast<FMODE == 2 ? 10 : 0>(fill_s ^ 4096u, outp_s, g0, quarter, lane, lc0, lc1);
-                else if (all_vec) seq_flush_quarter<false>(tile_ptr(fill_s ^ 4096u), pr, g0, quarter, lane, any_wasted);
-                else seq_flush_quarter<true>(tile_ptr(fill_s ^ 4096u), pr, g0, quarter, lane, any_wasted);
+                if (FMODE != 0) flush_quarter_fast<FMODE == 2 ? 10 : 0, OM>(fill_s ^ 4096u, outp_s, g0, quarter, lane, lc0, lc1);
+                else if (all_vec) seq_flush_quarter<false, OM>(tile_ptr(fill_s ^ 4096u), pr, g0, quarter, lane, any_wasted);
+                else seq_flush_quarter<true, OM>(tile_ptr(fill_s ^ 4096u), pr, g0, quarter, lane, any_wasted);
             }
             if (((t + 8) & 31) == 0) {
                 __syncwarp();
@@ -632,14 +689,14 @@ __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint
         if (have_drain) {  // whatever of the last full tile has not been written yet (re-writing a quarter is harmless)
             const uint32_t g0 = (bulk_end & ~31u) - 32;
 #pragma unroll
-            for (uint32_t i = 0; i < 4; i++) seq_flush_quarter<true>(tile_ptr(fill_s ^ 4096u), pr, g0, i, lane, any_wasted);
+            for (uint32_t i = 0; i < 4; i++) seq_flush_quarter<true, OM>(tile_ptr(fill_s ^ 4096u), pr, g0, i, lane, any_wasted);
         }
         __syncwarp();
 #pragma unroll
         for (int j = 0; j < TAPS; j++) h[j] = v[TAPS - 1 - j];
     }
     guarded(bulk_end, max_bs);
-    if (max_bs & 31) seq_flush<true>(tile_ptr(fill_s), pr, max_bs & ~31u, lane, any_wasted);
+    if (max_bs & 31) seq_flush<true, OM>(tile_ptr(fill_s), pr, max_bs & ~31u, lane, any_wasted);
 }
 
 // Two instances, launched back to back: GROUP 0 takes the warps whose largest predictor order is at most 12 (with
@@ -650,7 +707,11 @@ __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint
 // WIDE = true is the second chance of frames whose samples left the range the i32 accumulator is exact for (see
 // below): the same rows once more with the reference's i64 arithmetic only.  It looks at nothing unless the first
 // pass raised `need_wide`.
-template <int GROUP, bool WIDE>
+//
+// OM: the output mode (see SeqRow).  The interleaved instances write a frame's samples straight into the caller's
+// interleaved buffer `out`, after wasted bits and decorrelation as the planar flush applies them; the planar
+// instance is the one every other path shares.
+template <int GROUP, bool WIDE, int OM = CLX_OUT_PLANAR_I32>
 __global__ void __launch_bounds__(DEC_WARPS * 32)
 decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, const clx_frame_desc* __restrict__ descs,
                         uint32_t n_frames, int32_t* __restrict__ out, clx_frame_result* __restrict__ results,
@@ -675,7 +736,7 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
     int32_t* tile = s_tile[warp];
 
     bool active = false, narrow_ok = true, last = false;
-    uint32_t bs = 0, order = 0, shift = 0, wasted = 0, ca = 0, absum = 0, bit0 = 0, byte_len = 0;
+    uint32_t bs = 0, order = 0, shift = 0, wasted = 0, ca = 0, absum = 0, bit0 = 0, byte_len = 0, il_meta = 0;
     const SeqParams* sp = params;
     int32_t* sub = nullptr;
     SubLane<SubIO> L;
@@ -694,7 +755,12 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
             wasted = (uint32_t)sp->wasted;
             absum = sp->absum;
             ca = d.channel_assignment >= 8 ? d.channel_assignment : 0u;
-            sub = out + d.out_offset + (size_t)c * bs;
+            if constexpr (OM == CLX_OUT_PLANAR_I32) sub = out + d.out_offset + (size_t)c * bs;
+            else {  // the frame's first interleaved element
+                sub = reinterpret_cast<int32_t*>(reinterpret_cast<uint8_t*>(out) +
+                                                 d.out_offset * (OM == CLX_OUT_INTERLEAVED_I16 ? 2u : 4u));
+                il_meta = ((uint32_t)d.n_channels << 24) | (c << 28);
+            }
             uint32_t bits = d.bits_per_sample;  // nominal sample width (one extra bit for a side channel)
             if (d.channel_assignment == 9) bits += (c == 0);
             else if (d.channel_assignment == 8 || d.channel_assignment == 10) bits += (c == 1);
@@ -716,6 +782,7 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
         row.out = sub;
         row.bs = bs;
         row.meta = (vec_own ? 1u : 0u) | (wasted << 8) | ((c == 0 ? ca : 0u) << 16);
+        if constexpr (OM != CLX_OUT_PLANAR_I32) row.meta |= il_meta;
         pr[lane] = row;
         s_outp[warp][lane] = sub;
     }
@@ -727,12 +794,14 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
     // (with one channel slot per frame, rows 2p and 2p+1 are unrelated frames: mode 0)
     const uint32_t pair_ca = CH >= 2 ? __shfl_sync(0xffffffffu, ca, lane & ~1u) : 0u;
     const uint32_t ca0 = __shfl_sync(0xffffffffu, pair_ca, 0);
-    const bool fast_flush = __all_sync(0xffffffffu, active && vec_own && wasted == 0 && pair_ca == ca0);
+    // (interleaved: only stereo batches, whose row pairs are the two channels of one frame)
+    const bool fast_flush = (OM == CLX_OUT_PLANAR_I32 || CH == 2) &&
+                            __all_sync(0xffffffffu, active && vec_own && wasted == 0 && pair_ca == ca0);
     const int fmode = !fast_flush ? 0 : ca0 == 0 ? 1 : ca0 == 10 ? 2 : 0;
     int32_t smin = 0, smax = 0;
     const uint32_t tile_s = (uint32_t)__cvta_generic_to_shared(tile);
     const uint32_t outp_s = (uint32_t)__cvta_generic_to_shared(&s_outp[warp][0]);
-#define CLX_ROWS(T, UU, A, F) decode_rows<T, UU, A, F>(L, bs, order, shift, sp, active, tile, tile_s, pr, outp_s, lane, all_vec, any_wasted, smin, smax)
+#define CLX_ROWS(T, UU, A, F) decode_rows<T, UU, A, F, OM>(L, bs, order, shift, sp, active, tile, tile_s, pr, outp_s, lane, all_vec, any_wasted, smin, smax)
     // straight-line flush variants only where they pay: the i32-accumulator bodies (16-bit audio).  The i64 bodies are
     // what mixed batches run, several per SM at a time; there one body (12 taps, also for warps that would do with
     // 8) beats two that evict each other from the instruction cache.
@@ -803,7 +872,7 @@ size_t seq_scratch_bytes(const CoopPlan& plan, uint32_t n_frames) {
 
 cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
                        int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, void* d_params,
-                       const CoopPlan& plan, cudaStream_t stream, int which) {
+                       const CoopPlan& plan, cudaStream_t stream, int which, uint32_t mode) {
 #ifdef CLX_EXPERIMENT
     which &= g_exp_which;
 #endif
@@ -823,9 +892,16 @@ cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_fra
 #else
         const size_t dyn = 0;
 #endif
-#define CLX_DEC(C, W) decode_subframes_kernel<C, W><<<g2, b2, dyn, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, params, CH, ch_log2, n_pwarps, d_need_generic, d_need_generic + 2)
-        CLX_DEC(0, false); CLX_DEC(1, false);
-        if (!plan.no_wide) { CLX_DEC(0, true); CLX_DEC(1, true); }
+#define CLX_DEC(C, W, M) decode_subframes_kernel<C, W, M><<<g2, b2, dyn, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, params, CH, ch_log2, n_pwarps, d_need_generic, d_need_generic + 2)
+#define CLX_DEC4(M)                                                \
+    do {                                                           \
+        CLX_DEC(0, false, M); CLX_DEC(1, false, M);                \
+        if (!plan.no_wide) { CLX_DEC(0, true, M); CLX_DEC(1, true, M); } \
+    } while (0)
+        if (mode == CLX_OUT_INTERLEAVED_I16) CLX_DEC4(CLX_OUT_INTERLEAVED_I16);
+        else if (mode == CLX_OUT_INTERLEAVED_I32) CLX_DEC4(CLX_OUT_INTERLEAVED_I32);
+        else CLX_DEC4(CLX_OUT_PLANAR_I32);
+#undef CLX_DEC4
 #undef CLX_DEC
     }
     return cudaGetLastError();

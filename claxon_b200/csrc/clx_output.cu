@@ -15,13 +15,14 @@ constexpr uint32_t IL_TILE = 4096;  // interleaved elements per CTA
 
 // One CTA per (tile, frame).  Element i of a frame's interleaved block is sample t = i / n_channels of
 // channel c = i % n_channels, i.e. planar element c * block_size + t.  Writes are coalesced; the reads
-// are n_channels coalesced streams.
+// are n_channels coalesced streams.  `sel` / `gate` (optional, see launch_interleave) restrict it to some frames.
 template <int ESIZE>
 __global__ void __launch_bounds__(256)
 interleave_kernel(const clx_frame_desc* __restrict__ descs, uint32_t n_frames, const int32_t* __restrict__ planar,
-                  uint8_t* __restrict__ dst) {
+                  uint8_t* __restrict__ dst, const uint8_t* __restrict__ sel, const int* __restrict__ gate) {
+    if (gate != nullptr && *gate == 0) return;
     const uint32_t f = blockIdx.y;
-    if (f >= n_frames) return;
+    if (f >= n_frames || (sel != nullptr && sel[f] == 0)) return;
     const clx_frame_desc d = descs[f];
     const uint32_t nch = d.n_channels, bs = d.block_size, total = nch * bs;
     const uint32_t base = blockIdx.x * IL_TILE;
@@ -53,19 +54,35 @@ uint32_t output_elem_size(uint32_t mode) {
 }
 
 cudaError_t launch_interleave(const clx_frame_desc* d_descs, uint32_t n_frames, uint32_t max_frame_elems, const int32_t* d_planar,
-                              void* d_dst, uint32_t mode, cudaStream_t stream) {
+                              void* d_dst, uint32_t mode, cudaStream_t stream, const uint8_t* sel, const int* gate) {
     if (n_frames == 0 || mode == CLX_OUT_PLANAR_I32) return cudaSuccess;
     const uint32_t tiles = (max_frame_elems + IL_TILE - 1) / IL_TILE;
     for (uint32_t f0 = 0; f0 < n_frames; f0 += 65535) {  // gridDim.y limit
         const uint32_t nf = min(65535u, n_frames - f0);
         dim3 grid(tiles, nf);
+        const uint8_t* s = sel ? sel + f0 : nullptr;
         if (mode == CLX_OUT_INTERLEAVED_I16)
-            interleave_kernel<2><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (uint8_t*)d_dst);
+            interleave_kernel<2><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (uint8_t*)d_dst, s, gate);
         else if (mode == CLX_OUT_INTERLEAVED_I24)
-            interleave_kernel<3><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (uint8_t*)d_dst);
+            interleave_kernel<3><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (uint8_t*)d_dst, s, gate);
         else
-            interleave_kernel<4><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (uint8_t*)d_dst);
+            interleave_kernel<4><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (uint8_t*)d_dst, s, gate);
     }
+    return cudaGetLastError();
+}
+
+__global__ void __launch_bounds__(256)
+mark_status_kernel(const clx_frame_result* __restrict__ results, uint32_t n_frames, int32_t status, uint8_t* __restrict__ mark,
+                   const int* __restrict__ gate) {
+    if (*gate == 0) return;
+    const uint32_t f = blockIdx.x * 256 + threadIdx.x;
+    if (f < n_frames) mark[f] = results[f].status == status ? 1 : 0;
+}
+
+cudaError_t launch_mark_status(const clx_frame_result* d_results, uint32_t n_frames, int32_t status, uint8_t* d_mark,
+                               const int* gate, cudaStream_t stream) {
+    if (n_frames == 0) return cudaSuccess;
+    mark_status_kernel<<<(n_frames + 255) / 256, 256, 0, stream>>>(d_results, n_frames, status, d_mark, gate);
     return cudaGetLastError();
 }
 

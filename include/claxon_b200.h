@@ -212,16 +212,31 @@ int clx_batch_create(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const cl
 #define CLX_BATCH_BYTES_ON_DEVICE 1u
 int clx_batch_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
                         size_t n_frames, size_t out_elems, uint32_t batch_flags, clx_batch** out);
+/* Output modes for device-resident batches: the same batch with its samples kept in one of the CLX_OUT_* forms of
+ * clx_decode_frames_to, so that a consumer that stays on the device (clx_batch_device_out) gets what a WAV writer or
+ * the STREAMINFO MD5 uses without a conversion pass of its own.  `out_elems` and descs[i].out_offset count SAMPLES
+ * (elements of 2 / 3 / 4 bytes) as in clx_decode_frames_to, and the same rules hold: CLX_OUT_INTERLEAVED_I16 / _I24
+ * require every frame's bits_per_sample to be at most 16 / 24 (else CLX_ERR_INVALID_ARGUMENT, as for a mode above
+ * CLX_OUT_INTERLEAVED_I24), a sample that does not fit is truncated like `sample as i16`, and a failed frame's
+ * region is fully overwritten.  On the lane-per-frame path the I32 and I16 forms are written by the decode kernel
+ * itself; I24, and every other path, convert from planar inside the batch's graph.  clx_batch_create_ex is this call
+ * with CLX_OUT_PLANAR_I32. */
+int clx_batch_create_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
+                        size_t n_frames, size_t out_elems, uint32_t batch_flags, uint32_t mode, clx_batch** out);
 int clx_batch_decode(clx_ctx* ctx, clx_batch* b, uint32_t stream_index); /* async on an internal stream */
 int clx_batch_sync(clx_ctx* ctx, clx_batch* b);
+/* Planar batches only (CLX_ERR_INVALID_ARGUMENT for any other mode). */
 int clx_batch_read(clx_ctx* ctx, clx_batch* b, int32_t* out, size_t out_elems, clx_frame_result* results);
+/* Any mode: copies min(out_elems, the batch's out_elems) samples of the batch's own element size into `out` and the
+ * per-frame results (caller's frame order, CRC-16 verdicts applied) as clx_batch_read does. */
+int clx_batch_read_to(clx_ctx* ctx, clx_batch* b, void* out, size_t out_elems, clx_frame_result* results);
 void clx_batch_destroy(clx_ctx* ctx, clx_batch* b);
 /* Steady-state throughput: decodes `steps` batches back to back (step i = batches[i % n_batches]
  * on internal stream i % n_streams, so several batches are in flight) and returns the device time
  * from first launch to last completion, measured with CUDA events. */
 int clx_ctx_run_steps(clx_ctx* ctx, clx_batch** batches, size_t n_batches, uint32_t steps, uint32_t n_streams,
                       float* total_ms);
-/* Raw device pointers of a batch (for zero-copy consumers, e.g. torch / NCCL). */
+/* Raw device pointers of a batch (for zero-copy consumers, e.g. torch / NCCL); the output in the batch's mode. */
 void* clx_batch_device_out(clx_batch* b);
 void* clx_batch_device_bytes(clx_batch* b);
 /* Events-based timing of the kernels of the last `clx_batch_decode` on this batch (ms). */

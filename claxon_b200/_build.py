@@ -67,7 +67,7 @@ def build_lib(force: bool = False, verbose: bool = False) -> str:
         if os.path.exists(LIB):
             return LIB  # a machine without the CUDA toolkit: use the library built elsewhere
         raise RuntimeError("nvcc not found and no prebuilt libclaxon_b200.so")
-    extra = ["-DCLX_COOP_STATS"] if os.environ.get("CLX_COOP_STATS") else []
+    extra = []
     if os.environ.get("CLX_EXPERIMENT"):
         extra.append("-DCLX_EXPERIMENT")
     if os.environ.get("CLX_RING_TMA"):

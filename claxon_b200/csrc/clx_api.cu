@@ -94,11 +94,6 @@ struct clx_ctx {
     std::vector<cudaStream_t> streams;
     std::string last_error;
     uint64_t launches = 0;
-    int sm_count = 132;  // H100 SXM; replaced by the device's own count in clx_ctx_create
-    size_t smem_budget = 227 * 1024;
-    bool use_coop = true;
-    bool warp_per_frame = false;  // CLX_OPT_WARP_PER_FRAME: the warp-per-frame fast path (clx_coop.cu) everywhere
-    bool lane_per_frame_always = false;  // CLX_OPT_LANE_PER_FRAME: clx_fused.cu even for small synchronous calls
     // grow-only device scratch for clx_decode_frames, one set per stream (chunk pipelining)
     struct Scratch {
         uint8_t* d_bytes = nullptr; size_t bytes_cap = 0;
@@ -129,7 +124,7 @@ struct clx_batch {
     uint32_t n_frames = 0;
     cudaEvent_t ev_start = nullptr, ev_stop = nullptr;
     cudaStream_t last_stream = nullptr;
-    clx::CoopPlan plan;
+    clx::Plan plan;
     // The batch's launch sequence (flag reset + kernels) captured once as a CUDA graph: a decode is then
     // one graph launch instead of five stream operations, which matters when a step is ~25 us.
     cudaGraphExec_t graph = nullptr;
@@ -143,12 +138,11 @@ struct clx_batch {
     std::vector<uint32_t> order;   // device position -> caller's frame index (empty: identity), see shape_order()
     bool device_crc = false;       // bytes came from device memory: the CRC-16 check runs on the device, inside the graph
     // Output mode (CLX_OUT_*).  Interleaved batches hand out d_conv; d_out stays their planar scratch.  The lane-per-frame
-    // path writes I32 / I16 into d_conv itself (clx::FusedOut; d_mark: the frames the generic kernel took over); every
-    // other path, and I24, decodes to d_out and converts all frames inside the graph (launch_interleave).
+    // path writes I32 / I16 into d_conv itself (d_mark: the frames the generic kernel took over); every other path, and
+    // I24, decodes to d_out and converts all frames inside the graph (see clx::launch_decode).
     uint32_t mode = CLX_OUT_PLANAR_I32;
     void* d_conv = nullptr;
     uint8_t* d_mark = nullptr;
-    uint32_t max_frame_elems = 0;
 };
 
 namespace {
@@ -242,33 +236,31 @@ bool shape_order(const clx_frame_desc* descs, size_t lo, size_t hi, std::vector<
     return true;
 }
 
-// Chooses how a set of frames maps onto the cooperative kernel (frames per CTA, shared memory).
-// Two fast paths, two regimes.  The lane-per-frame path (clx_fused.cu) has the fewest instructions per
-// sample and is what a stream of batches should use; but a lane walks its whole frame alone, so one call
-// takes ~0.4 ms of device time however few frames it holds.  A synchronous host-buffer call with a few
-// thousand frames and nothing else in flight is latency-bound: there the warp-per-frame path
-// (clx_coop.cu: 32 lanes share a frame, ~0.25 ms per 1024 frames) finishes sooner and lets the PCM
-// copy-out start earlier.  `latency_call` = the plan is for such a call.
+// Chooses the decode path of a set of frames.  Two fast paths, two regimes.  The lane-per-frame path (clx_fused.cu)
+// has the fewest instructions per sample and is what a stream of batches should use; but a lane walks its whole frame
+// alone, so one call takes ~0.4 ms of device time however few frames it holds.  A synchronous host-buffer call with a
+// few thousand frames and nothing else in flight is latency-bound: there the warp-per-frame path (clx_coop.cu: 32 lanes
+// share a frame, ~0.25 ms per 1024 frames) finishes sooner and lets the PCM copy-out start earlier.  `latency_call` =
+// the plan is for such a call.
+// (Frames with many channels and long blocks — BASELINE.json's stress shape, 8 x 16384 — are latency-bound on either
+// fast path: the index lane walks (channels - 1) * block_size Rice codes alone.  No special case.)
 constexpr size_t kLatencyRegimeFrames = 4096;
-clx::CoopPlan make_plan(const clx_ctx* ctx, const clx_frame_desc* descs, size_t n, bool latency_call = false) {
-    clx::CoopPlan plan;
+clx::Plan make_plan(const clx_ctx* ctx, const clx_frame_desc* descs, size_t n, bool latency_call = false) {
+    clx::Plan plan;
     plan.no_generic = (ctx->flags & CLX_OPT_NO_GENERIC) != 0;
     plan.no_wide = (ctx->flags & CLX_OPT_NO_WIDE) != 0;
-    if (!ctx->use_coop) return plan;
-    uint32_t max_elems = 0, max_ch = 0, max_bs = 0, max_bps = 0;
+    uint32_t max_ch = 0;
     for (size_t i = 0; i < n; i++) {
-        max_elems = std::max<uint32_t>(max_elems, (uint32_t)descs[i].n_channels * descs[i].block_size);
+        plan.max_frame_elems = std::max<uint32_t>(plan.max_frame_elems, (uint32_t)descs[i].n_channels * descs[i].block_size);
         max_ch = std::max<uint32_t>(max_ch, descs[i].n_channels);
-        max_bs = std::max<uint32_t>(max_bs, descs[i].block_size);
-        max_bps = std::max<uint32_t>(max_bps, descs[i].bits_per_sample);
     }
-    // (Frames with many channels and long blocks — BASELINE.json's stress shape, 8 x 16384 — are latency-bound on
-    // either fast path: the index lane walks (channels - 1) * block_size Rice codes alone.  No special case.)
-    if (clx::coop_plan(max_elems, max_ch, (uint32_t)n, ctx->sm_count, ctx->smem_budget, &plan) && !ctx->warp_per_frame &&
-        !(latency_call && !ctx->lane_per_frame_always)) {
-        plan.G = 2;
-        plan.max_bs = max_bs;
-    }
+    if ((ctx->flags & CLX_OPT_GENERIC_KERNEL_ONLY) || n == 0 || max_ch > 8) return plan;
+    plan.channels = 1;
+    while (plan.channels < max_ch) plan.channels <<= 1;  // a power of two, so that a warp holds whole frames
+    if ((ctx->flags & CLX_OPT_WARP_PER_FRAME) || (latency_call && !(ctx->flags & CLX_OPT_LANE_PER_FRAME)))
+        plan.path = clx::Path::WarpPerFrame;
+    else
+        plan.path = clx::Path::LanePerFrame;
     return plan;
 }
 
@@ -296,14 +288,6 @@ int clx_ctx_create(const clx_options* opts, clx_ctx** out) {
             return CLX_ERR_CUDA;
         }
     ctx->scratch.resize(ns);
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, ctx->device) == cudaSuccess) {
-        ctx->sm_count = prop.multiProcessorCount;
-        ctx->smem_budget = prop.sharedMemPerBlockOptin;
-    }
-    if (opts && (opts->flags & CLX_OPT_GENERIC_KERNEL_ONLY)) ctx->use_coop = false;
-    if (opts && (opts->flags & CLX_OPT_WARP_PER_FRAME)) ctx->warp_per_frame = true;
-    if (opts && (opts->flags & CLX_OPT_LANE_PER_FRAME)) ctx->lane_per_frame_always = true;
     ctx->host_threads = std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
     if (opts && opts->host_threads) ctx->host_threads = std::max(1u, std::min(64u, opts->host_threads));
     *out = ctx;
@@ -424,27 +408,20 @@ int clx_decode_frames_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, cons
         if ((rc = grow(ctx, sc.d_out, sc.out_cap, lead + no + 4, 4096))) return drain(rc);
         if ((rc = grow(ctx, sc.d_results, sc.results_cap, nf, 64))) return drain(rc);
         if (!sc.d_need_hi) CUD(cudaMalloc((void**)&sc.d_need_hi, 4 * sizeof(int)));
-        const clx::CoopPlan plan = make_plan(ctx, descs + s.f0, nf, n_frames <= kLatencyRegimeFrames);
+        const clx::Plan plan = make_plan(ctx, descs + s.f0, nf, n_frames <= kLatencyRegimeFrames);
         if ((rc = grow(ctx, sc.d_params, sc.params_cap, clx::coop_params_bytes(plan, (uint32_t)nf) + 16, 4096))) return drain(rc);
         if (mode != CLX_OUT_PLANAR_I32 && (rc = grow(ctx, sc.d_conv, sc.conv_cap, (lead + no + 4) * esize, 4096))) return drain(rc);
         enqueued = c + 1;
         CUD(cudaMemcpyAsync(sc.d_bytes, bytes + s.b0, nb, cudaMemcpyHostToDevice, st));
         CUD(cudaMemcpyAsync(sc.d_descs, ctx->h_descs + s.f0, nf * sizeof(clx_frame_desc), cudaMemcpyHostToDevice, st));
-        CUD(clx::launch_decode(sc.d_bytes, nb_pad, sc.d_descs, (uint32_t)nf, sc.d_out, sc.d_results, sc.d_need_hi,
-                               sc.d_params, plan, st, &ctx->launches));
-        if (!(ctx->flags & CLX_OPT_NO_VERIFY_CRC)) {  // src/frame.rs:752-763, after the subframes, on the device
-            CUD(clx::launch_crc16(sc.d_bytes, sc.d_descs, (uint32_t)nf, sc.d_results, st));
-            ctx->launches++;
-        }
-        if (mode == CLX_OUT_PLANAR_I32) {
+        // (never fused: no d_mark; the frame CRC-16 on the device, src/frame.rs:752-763)
+        const clx::DecodeBuffers db{sc.d_bytes, nb_pad, sc.d_descs, (uint32_t)nf, sc.d_out, sc.d_results, sc.d_need_hi,
+                                    sc.d_params, mode, sc.d_conv, nullptr};
+        CUD(clx::launch_decode(db, plan, !(ctx->flags & CLX_OPT_NO_VERIFY_CRC), st, &ctx->launches));
+        if (mode == CLX_OUT_PLANAR_I32)
             CUD(cudaMemcpyAsync(out + s.o0 * esize, sc.d_out + lead, no * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        } else {
-            uint32_t max_elems = 0;
-            for (size_t i = s.f0; i < s.f1; i++) max_elems = std::max<uint32_t>(max_elems, (uint32_t)descs[i].n_channels * descs[i].block_size);
-            CUD(clx::launch_interleave(sc.d_descs, (uint32_t)nf, max_elems, sc.d_out, sc.d_conv, mode, st));
-            ctx->launches++;
+        else
             CUD(cudaMemcpyAsync(out + s.o0 * esize, sc.d_conv + lead * esize, no * esize, cudaMemcpyDeviceToHost, st));
-        }
         CUD(cudaMemcpyAsync(ctx->h_results + s.f0, sc.d_results, nf * sizeof(clx_frame_result), cudaMemcpyDeviceToHost, st));
     }
 #ifdef CLX_EXPERIMENT
@@ -496,8 +473,6 @@ int clx_batch_create_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const
     b->n_frames = (uint32_t)n_frames;
     b->plan = make_plan(ctx, descs, n_frames);
     b->mode = mode;
-    for (size_t i = 0; i < n_frames; i++)
-        b->max_frame_elems = std::max<uint32_t>(b->max_frame_elems, (uint32_t)descs[i].n_channels * descs[i].block_size);
     cudaError_t e = cudaMalloc((void**)&b->d_bytes, b->buf_bytes);
     if (e == cudaSuccess) e = cudaMemset(b->d_bytes, 0, b->buf_bytes);
     if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_descs, std::max<size_t>(1, n_frames) * sizeof(clx_frame_desc));
@@ -539,22 +514,10 @@ int clx_batch_create_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const
 }  // extern "C"
 
 namespace {
-// The launch sequence of one decode of a batch: the decode kernels, the device CRC-16 (bytes from device memory),
-// and the conversion to the batch's interleaved mode where the decode pass does not write that mode itself.
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
-    const bool fused = (b->mode == CLX_OUT_INTERLEAVED_I32 || b->mode == CLX_OUT_INTERLEAVED_I16) && b->plan.G == 2;
-    const clx::FusedOut fo{b->mode, b->d_conv, b->d_mark, b->max_frame_elems};
-    cudaError_t e = clx::launch_decode(b->d_bytes, b->buf_bytes, b->d_descs, b->n_frames, b->d_out, b->d_results, b->d_need_hi,
-                                       b->d_params, b->plan, st, launches, fused ? &fo : nullptr);
-    if (e == cudaSuccess && b->device_crc) {
-        e = clx::launch_crc16(b->d_bytes, b->d_descs, b->n_frames, b->d_results, st);
-        (*launches)++;
-    }
-    if (e == cudaSuccess && b->mode != CLX_OUT_PLANAR_I32 && !fused) {
-        e = clx::launch_interleave(b->d_descs, b->n_frames, b->max_frame_elems, b->d_out, b->d_conv, b->mode, st);
-        (*launches)++;
-    }
-    return e;
+    const clx::DecodeBuffers db{b->d_bytes, b->buf_bytes, b->d_descs, b->n_frames, b->d_out, b->d_results, b->d_need_hi,
+                                b->d_params, b->mode, b->d_conv, b->d_mark};
+    return clx::launch_decode(db, b->plan, b->device_crc, st, launches);
 }
 
 // Captures the batch's launch sequence once; called from clx_batch_create so that no decode ever pays for

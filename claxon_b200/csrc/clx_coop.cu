@@ -37,6 +37,7 @@
 #include <cstdlib>
 
 #include "clx_internal.h"
+#include "clx_lanes.h"
 
 namespace clx {
 
@@ -57,7 +58,6 @@ struct SubParams {   // one per subframe (global memory, written by the entropy 
 // ahead with a single coalesced 16-byte load per lane and nothing touches it until it slides into
 // X, so HBM/L2 latency stays off the critical path.  All field extraction is shuffle + funnel shift.
 // ---------------------------------------------------------------------------------
-__device__ unsigned long long g_coop_stats[16];  // debug counters
 constexpr uint32_t WPL = 4;            // words per lane
 constexpr uint32_t STAGE_CODES = 1024;  // codes one window may emit (a window with more is cut short)
 constexpr uint32_t WIN_WORDS = 32 * WPL;
@@ -71,7 +71,6 @@ struct Win {
     uint32_t pending;
 };
 
-__device__ __forceinline__ uint32_t bswap32(uint32_t v) { return __byte_perm(v, 0, 0x0123); }
 __device__ __forceinline__ uint4 win_ldg(const Win& w, uint32_t quad) {
     uint4 v = make_uint4(0, 0, 0, 0);
     if (quad < w.qlim) v = __ldg(w.base + quad);
@@ -80,7 +79,7 @@ __device__ __forceinline__ uint4 win_ldg(const Win& w, uint32_t quad) {
 __device__ __forceinline__ void win_prime(Win& w, uint32_t bitpos, uint32_t lane) {
     w.b0 = (bitpos >> 5) & ~3u;
     const uint4 x = win_ldg(w, (w.b0 >> 2) + lane), y = win_ldg(w, (w.b0 >> 2) + 32 + lane);
-    w.X[0] = bswap32(x.x); w.X[1] = bswap32(x.y); w.X[2] = bswap32(x.z); w.X[3] = bswap32(x.w);
+    w.X[0] = hd_bswap(x.x); w.X[1] = hd_bswap(x.y); w.X[2] = hd_bswap(x.z); w.X[3] = hd_bswap(x.w);
     w.Y[0] = y.x; w.Y[1] = y.y; w.Y[2] = y.z; w.Y[3] = y.w;
     w.pending = 0;
 }
@@ -103,7 +102,7 @@ __device__ __forceinline__ void win_advance(Win& w, uint32_t bitpos, uint32_t la
     for (uint32_t j = 0; j < WPL; j++) {
         const uint32_t xs = __shfl_sync(0xffffffffu, w.X[j], src);
         const uint32_t ys = __shfl_sync(0xffffffffu, w.Y[j], src);
-        w.X[j] = low ? xs : bswap32(ys);
+        w.X[j] = low ? xs : hd_bswap(ys);
         w.Y[j] = ys;  // lanes with !low get their real Y from F at the next slide
     }
     w.pending = low ? 0u : 1u;
@@ -138,9 +137,6 @@ __device__ __forceinline__ uint32_t win_peek32_lane(const Win& w, uint32_t bitpo
     const uint32_t w0 = (i & 3) == 0 ? a[0] : (i & 3) == 1 ? a[1] : (i & 3) == 2 ? a[2] : a[3];
     const uint32_t w1 = (i1 & 3) == 0 ? b[0] : (i1 & 3) == 1 ? b[1] : (i1 & 3) == 2 ? b[2] : b[3];
     return __funnelshift_l(w1, w0, bitpos & 31);
-}
-__device__ __forceinline__ int32_t sext(uint32_t v, uint32_t bits) {
-    return ((int32_t)(v << (32 - bits))) >> (32 - bits);
 }
 
 // ---------------------------------------------------------------------------------
@@ -311,17 +307,6 @@ __device__ __forceinline__ uint32_t rice_window(const Win& w, uint32_t& P, uint3
     return total;
 }
 
-// Inter-channel decorrelation of one (ch0, ch1) pair; wrapping i32 (src/frame.rs:319-389).
-__device__ __forceinline__ void decor(uint32_t ca, int32_t a, int32_t b, int32_t& o0, int32_t& o1) {
-    if (ca == 8) { o0 = a; o1 = (int32_t)((uint32_t)a - (uint32_t)b); }
-    else if (ca == 9) { o0 = (int32_t)((uint32_t)a + (uint32_t)b); o1 = b; }
-    else {  // (mid*2 | side&1) +- side is even, so the reference's `/ 2` equals `>> 1`
-        const uint32_t m = ((uint32_t)a << 1) | ((uint32_t)b & 1u);
-        o0 = ((int32_t)(m + (uint32_t)b)) >> 1;
-        o1 = ((int32_t)(m - (uint32_t)b)) >> 1;
-    }
-}
-
 // Per-lane, branch-free form for the predict kernel: the lane holds one channel's sample `own`, its
 // neighbour's is `other`.  Every case of src/frame.rs:319-389 is (own*p + other*q + side&1) >> s in
 // wrapping i32 with per-lane constants (side = channel 1's sample):
@@ -348,7 +333,6 @@ __device__ __forceinline__ int32_t decor_lane(uint32_t own, uint32_t other, cons
 
 constexpr int ENT_WARPS = 4;   // entropy kernel: frames (warps) per CTA
 constexpr int PRE_WARPS = 2;   // predict kernel: warps per CTA
-constexpr int COOP_MAX_CH = 8;
 constexpr int RING_SAMPLES = 64;                 // predict kernel: residual ring per lane
 constexpr int RING_LANE_WORDS = RING_SAMPLES + 4; // +16 bytes of skew: 16-byte accesses of 8 lanes hit 32 banks
 
@@ -410,7 +394,7 @@ entropy_frames_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, con
         if ((type == 2 || type == 3) && order > bs) { ok = false; break; }
         if (lane == 0) { sp->order = 0; sp->shift = 0; sp->wasted = (int32_t)wasted; sp->narrow = 0; }
         if (type == 0) {  // constant (src/subframe.rs:382-394)
-            const int32_t v = sext(top_bits(win_peek32(w, P), sfbps), sfbps);
+            const int32_t v = hd_sext(top_bits(win_peek32(w, P), sfbps), sfbps);
             P += sfbps;
             for (uint32_t i = lane; i < bs; i += 32) sbuf[i] = v;
             if (P > limit) { ok = false; break; }
@@ -422,7 +406,7 @@ entropy_frames_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, con
             win_advance(w, P, lane);
             const uint32_t i = i0 + lane;
             const uint32_t v = win_peek32_lane(w, P + lane * sfbps);
-            if (i < n_raw) sbuf[i] = sext(top_bits(v, sfbps), sfbps);
+            if (i < n_raw) sbuf[i] = hd_sext(top_bits(v, sfbps), sfbps);
             P += min(32u, n_raw - i0) * sfbps;
         }
         if (P > limit) { ok = false; break; }
@@ -436,17 +420,14 @@ entropy_frames_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, con
             const uint32_t prec_m1 = pq >> 5;
             if (prec_m1 == 15) { ok = false; break; }
             const uint32_t precision = prec_m1 + 1;
-            const int32_t sh = sext(pq & 31u, 5);
+            const int32_t sh = hd_sext(pq & 31u, 5);
             if (sh < 0) { ok = false; break; }
             shift = (uint32_t)sh;
             const uint32_t v = win_peek32_lane(w, P + lane * precision);
-            if (lane < order) sp->coefs[lane] = (int16_t)sext(top_bits(v, precision), precision);
+            if (lane < order) sp->coefs[lane] = (int16_t)hd_sext(top_bits(v, precision), precision);
             P += order * precision;
         } else if (lane < 4) {
-            // row `order` of {1}, {2,-1}, {3,-3,1}, {4,-6,4,-1}; coefs[0] multiplies s[t-1]
-            const uint32_t packed = order == 1 ? 0x00000001u : order == 2 ? 0x0000ff02u
-                                  : order == 3 ? 0x0001fd03u : order == 4 ? 0xff04fa04u : 0u;
-            sp->coefs[lane] = (int16_t)(int8_t)(packed >> (8 * lane));
+            sp->coefs[lane] = (int16_t)(int8_t)(fixed_coefs_packed(order) >> (8 * lane));
         }
         if (lane == 0) { sp->order = (int32_t)order; sp->shift = (int32_t)shift; }
         // ---- residual (src/subframe.rs:236-380) ----
@@ -496,48 +477,11 @@ entropy_frames_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, con
 // ---------------------------------------------------------------------------------
 // Kernel 2: prediction + wasted shift + decorrelation, one lane per subframe, in place
 // ---------------------------------------------------------------------------------
-// One trip of the recurrence for U consecutive samples.  v[0..TAPS) = history (oldest first),
-// v[TAPS+i] = sample i of this trip.  Terms that only involve history are summed first (they do not
-// depend on this trip's samples), the terms with fresh samples last, most recent last — the serial
-// chain per sample is then one multiply-add, the shift and the residual add.
-//
-// ACC = long long is the reference's arithmetic verbatim (i64 products and sum).  ACC = int is the same
-// recurrence with 32-bit wrapping multiply-adds — 2.3x cheaper on this chip — and yields bit-identical
-// samples whenever no sum of products leaves the i32 range, i.e. whenever
-// sum|coef| * max|sample| < 2^31: it is chosen only where a valid stream guarantees that, and the
-// condition is re-checked against the samples actually produced (if it ever fails the frame is
-// re-decoded by the generic kernel, so the output never depends on the shortcut).
-template <int TAPS, int U, typename ACC>
-__device__ __forceinline__ void predict_trip(int32_t (&v)[TAPS + U], const int32_t (&c)[TAPS], const int32_t (&r)[U],
-                                             uint32_t shift) {
-    ACC part[U];
-#pragma unroll
-    for (int i = 0; i < U; i++) {
-        ACC acc = 0;
-#pragma unroll
-        for (int j = 0; j < TAPS; j++)  // c[j] multiplies v[i + TAPS - 1 - j]; history only here
-            if (i + TAPS - 1 - j < TAPS) acc += (ACC)c[j] * (ACC)v[i + TAPS - 1 - j];
-        part[i] = acc;
-    }
-#pragma unroll
-    for (int i = 0; i < U; i++) {
-        ACC acc = part[i];
-#pragma unroll
-        for (int j = TAPS - 1; j >= 0; j--)  // fresh samples, oldest first
-            if (i + TAPS - 1 - j >= TAPS) acc += (ACC)c[j] * (ACC)v[i + TAPS - 1 - j];
-        v[TAPS + i] = (int32_t)(acc >> shift) + r[i];
-    }
-}
-
 struct PredRow {       // per lane, shared memory: where the lane's samples go
     int32_t* out;      // subframe's first output element (nullptr: idle lane)
     uint32_t bs;       // block size
     uint32_t vec_ok;   // 16-byte stores allowed
 };
-
-__device__ __forceinline__ uint32_t tile_word(uint32_t row, uint32_t col) {
-    return row * 32 + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3));
-}
 
 // Writes the warp's 32x32 tile (steps [g0, g0+32) of every lane's subframe) to global memory.
 __device__ __forceinline__ void flush_rows(const int32_t* tile, const PredRow* rows, uint32_t g0, uint32_t lane) {
@@ -641,7 +585,7 @@ __device__ __forceinline__ void predict_rows(const int32_t* __restrict__ src, ui
                 const int4 x = *reinterpret_cast<const int4*>(ring + (trip % SLOTS) * U + 4 * q);
                 r[4 * q] = x.x; r[4 * q + 1] = x.y; r[4 * q + 2] = x.z; r[4 * q + 3] = x.w;
             }
-            predict_trip<TAPS, U, ACC>(v, c, r, shift);
+            seq_trip<TAPS, U, ACC>(v, c, r, shift);
 #pragma unroll
             for (int i = 0; i < U; i++) {
                 smin = min(smin, v[TAPS + i]);
@@ -707,7 +651,7 @@ predict_frames_kernel(const clx_frame_desc* __restrict__ descs, uint32_t n_frame
             if (d.channel_assignment == 9) bits += (c == 0);
             else if (d.channel_assignment == 8 || d.channel_assignment == 10) bits += (c == 1);
             // valid streams keep |sample| <= 2^(bits-1); anything beyond is caught by the check below
-            narrow_ok = ((unsigned long long)absum << (bits - 1)) < (1ull << 31);
+            narrow_ok = i32_acc_exact(absum, bits);
         }
     }
     PredRow pr;
@@ -747,47 +691,29 @@ predict_frames_kernel(const clx_frame_desc* __restrict__ descs, uint32_t n_frame
 // ---------------------------------------------------------------------------------
 // launch helpers
 // ---------------------------------------------------------------------------------
-bool coop_plan(uint32_t max_frame_elems, uint32_t max_channels, uint32_t n_frames, int sm_count, size_t smem_budget,
-               CoopPlan* plan) {
-    (void)sm_count; (void)smem_budget;
-    plan->G = 0;
-    if (max_frame_elems == 0 || n_frames == 0 || max_channels == 0 || max_channels > COOP_MAX_CH) return false;
-    uint32_t ch = 1;
-    while (ch < max_channels) ch <<= 1;  // channel slots per frame: a power of two, so a warp holds whole frames
-    plan->G = 1;
-    plan->channels = ch;
-    plan->frame_stride = 0;
-    plan->smem_bytes = 0;
-    return true;
+size_t coop_params_bytes(const Plan& plan, uint32_t n_frames) {
+    switch (plan.path) {
+        case Path::LanePerFrame: return seq_scratch_bytes(plan, n_frames);
+        case Path::WarpPerFrame: return (size_t)n_frames * plan.channels * sizeof(SubParams);
+        case Path::Generic: break;
+    }
+    return 0;
 }
 
-size_t coop_params_bytes(const CoopPlan& plan, uint32_t n_frames) {
-    if (plan.G == 2) return seq_scratch_bytes(plan, n_frames);
-    return plan.G ? (size_t)n_frames * plan.channels * sizeof(SubParams) : 0;
-}
-
-cudaError_t launch_coop(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
-                        int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, void* d_params,
-                        const CoopPlan& plan, cudaStream_t stream, uint32_t mode) {
-    if (plan.G == 2)
-        return launch_seq(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, d_need_generic, d_params, plan, stream, 3, mode);
+cudaError_t launch_warp_per_frame(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
+                                  int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, void* d_params,
+                                  const Plan& plan, cudaStream_t stream, uint64_t* launches) {
     SubParams* params = reinterpret_cast<SubParams*>(d_params);
     const uint32_t CH = plan.channels;
     dim3 g1((n_frames + ENT_WARPS - 1) / ENT_WARPS), b1(ENT_WARPS * 32);
     entropy_frames_kernel<<<g1, b1, 0, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, params, CH,
                                                  d_need_generic);
+    (*launches)++;
     const uint64_t slots = (uint64_t)n_frames * CH;
     dim3 g2((uint32_t)((slots + PRE_WARPS * 32 - 1) / (PRE_WARPS * 32))), b2(PRE_WARPS * 32);
     predict_frames_kernel<<<g2, b2, 0, stream>>>(d_descs, n_frames, d_out, d_results, params, CH, d_need_generic);
+    (*launches)++;
     return cudaGetLastError();
 }
 
-
 }  // namespace clx
-
-#ifdef CLX_COOP_STATS
-extern "C" void clx_debug_coop_stats(unsigned long long* out16, int reset) {
-    cudaMemcpyFromSymbol(out16, clx::g_coop_stats, sizeof(unsigned long long) * 16);
-    if (reset) { unsigned long long z[16] = {0}; cudaMemcpyToSymbol(clx::g_coop_stats, z, sizeof z); }
-}
-#endif

@@ -127,10 +127,11 @@ cudaError_t crc16_init() {
 }
 
 cudaError_t launch_crc16(const uint8_t* d_bytes, const clx_frame_desc* d_descs, uint32_t n_frames, clx_frame_result* d_results,
-                         cudaStream_t stream) {
+                         cudaStream_t stream, uint64_t* launches) {
     if (n_frames == 0) return cudaSuccess;
     static const CrcPowers pw = host_powers();
     crc16_frames_kernel<<<(n_frames + CRC_WARPS - 1) / CRC_WARPS, CRC_WARPS * 32, 0, stream>>>(d_bytes, d_descs, n_frames, d_results, pw);
+    (*launches)++;
     return cudaGetLastError();
 }
 

@@ -30,6 +30,7 @@
 
 #include "claxon_b200.h"
 #include "clx_internal.h"
+#include "clx_lanes.h"
 
 namespace clx {
 
@@ -159,9 +160,6 @@ __device__ __forceinline__ uint32_t bc_read(BitCur& b, uint32_t n) {  // n <= 32
     bc_skip(b, n);
     return v;
 }
-__device__ __forceinline__ int32_t sign_extend(uint32_t v, uint32_t bits) {  // src/subframe.rs:117-122
-    return ((int32_t)(v << (32 - bits))) >> (32 - bits);
-}
 // Unary run of any length (src/input.rs:475-511); stops counting once past `limit_bits`.
 __device__ __forceinline__ uint32_t bc_unary_slow(BitCur& b, uint32_t limit_bits) {
     uint32_t q = 0;
@@ -189,10 +187,6 @@ struct RowInfo {      // per lane/frame, constant for the kernel
     uint32_t total;   // n_channels * block_size
     uint32_t bs_mode; // block_size | channel_assignment << 16 | vec_ok << 24
 };
-
-__device__ __forceinline__ uint32_t tile_word(uint32_t row, uint32_t col) {
-    return row * 32 + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3));
-}
 
 // Inter-channel decorrelation of one (ch0, ch1) pair; wrapping i32 (src/frame.rs:319-389).
 __device__ __forceinline__ void decorrelate(uint32_t ca, int32_t a, int32_t b, int32_t& o0, int32_t& o1) {
@@ -364,7 +358,7 @@ __device__ __forceinline__ void parse_subframe_header(Lane<KORD>& L, int* need_h
 #pragma unroll
     for (int j = 0; j < KORD; j++) L.c[j] = 0;
     if (type == 0) {
-        L.cval = sign_extend(bc_read(b, L.sfbps), L.sfbps);
+        L.cval = hd_sext(bc_read(b, L.sfbps), L.sfbps);
         L.mode = M_CONST;
         if (overrun(L)) return fail(L, CLX_ERR_IO_UNEXPECTED_EOF);
     } else if (type == 1) {
@@ -406,14 +400,14 @@ __device__ __forceinline__ void parse_params(Lane<KORD>& L) {
         uint32_t prec_m1 = pq >> 5;
         if (prec_m1 == 15) return fail_at(L, CLX_ERR_QLP_PRECISION_INVALID, p0 + 4);
         uint32_t precision = prec_m1 + 1;
-        int32_t shift = sign_extend(pq & 31u, 5);
+        int32_t shift = hd_sext(pq & 31u, 5);
         if (shift < 0) return fail(L, CLX_ERR_NEGATIVE_QLP_SHIFT);
         L.shift = (uint32_t)shift;
         // First coefficient in the stream multiplies the most recent sample (:696-701).
 #pragma unroll
         for (int j = KORD - 1; j >= 0; j--) {
             if ((uint32_t)(KORD - 1 - j) < L.order)
-                L.c[j] = sign_extend(bc_read(b, precision), precision);
+                L.c[j] = hd_sext(bc_read(b, precision), precision);
         }
     } else {
         L.shift = 0;
@@ -664,7 +658,7 @@ decode_frames_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes,
                     s = (int32_t)(acc >> L.shift) + e;
                     L.rem--;
                 } else if (L.mode == M_VERB) {
-                    s = sign_extend(bc_read(L.bc, L.sfbps), L.sfbps);
+                    s = hd_sext(bc_read(L.bc, L.sfbps), L.sfbps);
                 } else {
                     s = L.cval;
                 }
@@ -687,48 +681,57 @@ decode_frames_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes,
 // ---------------------------------------------------------------------------------
 // launch
 // ---------------------------------------------------------------------------------
-cudaError_t launch_decode(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs,
-                          uint32_t n_frames, int32_t* d_out, clx_frame_result* d_results, int* d_flags,
-                          void* d_params, const CoopPlan& plan, cudaStream_t stream, uint64_t* launches,
-                          const FusedOut* fused) {
-    if (n_frames == 0) return cudaSuccess;
-    const uint32_t per_cta = WARPS_PER_CTA * 32;
-    dim3 grid((n_frames + per_cta - 1) / per_cta), block(per_cta);
-    int* d_generic = d_flags;      // set by the cooperative kernel: some frames need the generic kernel
-    int* d_need_hi = d_flags + 1;  // set by the 12-tap generic instance: some frames need 32 taps
-    cudaError_t e = cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream);  // [0] generic, [1] 32 taps, [2] i64 retry
+cudaError_t launch_decode(const DecodeBuffers& b, const Plan& plan, bool crc, cudaStream_t stream, uint64_t* launches) {
+    if (b.n_frames == 0) return cudaSuccess;
+    const bool fast = plan.path != Path::Generic;
+    // The lane-per-frame decode pass writes interleaved I32 / I16 itself when the caller keeps the frames to convert
+    // after the generic kernel (`mark`); every other path, and I24, decodes to planar and converts all frames at the end.
+    const bool fused = plan.path == Path::LanePerFrame && b.mark != nullptr &&
+                       (b.mode == CLX_OUT_INTERLEAVED_I32 || b.mode == CLX_OUT_INTERLEAVED_I16);
+    int* d_generic = b.flags;        // set by a fast path: some frames need the generic kernel
+    int* d_need_hi = b.flags + 1;    // set by the 12-tap generic instance: some frames need 32 taps
+    int* d_need_wide = b.flags + 2;  // set by the lane-per-frame decode pass: some frames need the i64 second chance
+    cudaError_t e = cudaMemsetAsync(b.flags, 0, 4 * sizeof(int), stream);
     if (e != cudaSuccess) return e;
-    if (plan.G > 0 && d_params != nullptr) {
-        if (fused) e = launch_coop(d_bytes, buf_bytes, d_descs, n_frames, static_cast<int32_t*>(fused->d_dst), d_results, d_generic,
-                                   d_params, plan, stream, fused->mode);
-        else e = launch_coop(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, d_generic, d_params, plan, stream);
-        if (e != cudaSuccess) return e;
-        // index pass + two decode instances (+ two WIDE ones) / entropy + prediction
-        if (launches) *launches += plan.G == 2 ? (plan.no_wide ? 3 : 5) : 2;
-        if (plan.no_generic) return cudaGetLastError();  // testing: leave the fast path's verdicts as they are
+    if (plan.path == Path::LanePerFrame)
+        e = launch_seq(b.bytes, b.buf_bytes, b.descs, b.n_frames, fused ? static_cast<int32_t*>(b.conv) : b.out, b.results,
+                       d_generic, d_need_wide, b.params, plan, fused ? b.mode : (uint32_t)CLX_OUT_PLANAR_I32, stream, launches);
+    else if (plan.path == Path::WarpPerFrame)
+        e = launch_warp_per_frame(b.bytes, b.buf_bytes, b.descs, b.n_frames, b.out, b.results, d_generic, b.params, plan,
+                                  stream, launches);
+    if (e != cudaSuccess) return e;
+    if (!(fast && plan.no_generic)) {  // (testing: no_generic leaves the fast path's verdicts as they are)
         if (fused) {  // the frames the generic kernel is about to take over, whatever the fast path wrote for them
-            e = launch_mark_status(d_results, n_frames, CLX_INTERNAL_NEED_GENERIC, fused->d_mark, d_generic, stream);
+            e = launch_mark_status(b.results, b.n_frames, CLX_INTERNAL_NEED_GENERIC, b.mark, d_generic, stream, launches);
             if (e != cudaSuccess) return e;
-            if (launches) *launches += 1;
         }
-        decode_frames_kernel<12><<<grid, block, 0, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results,
-                                                             d_need_hi, d_generic, CLX_INTERNAL_NEED_GENERIC);
-    } else {
-        decode_frames_kernel<12><<<grid, block, 0, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results,
-                                                             d_need_hi, nullptr, 0);
+        const uint32_t per_cta = WARPS_PER_CTA * 32;
+        dim3 grid((b.n_frames + per_cta - 1) / per_cta), block(per_cta);
+        // After a fast path: only the frames it declined, and nothing at all when it declined none.
+        decode_frames_kernel<12><<<grid, block, 0, stream>>>(b.bytes, b.buf_bytes, b.descs, b.n_frames, b.out, b.results,
+                                                             d_need_hi, fast ? d_generic : nullptr,
+                                                             fast ? CLX_INTERNAL_NEED_GENERIC : 0);
+        (*launches)++;
+        // Frames with an LPC order above 12 (non-subset streams) were only flagged by the 12-tap
+        // instance; the 32-tap instance picks them up.  It exits immediately when nothing was flagged.
+        decode_frames_kernel<32><<<grid, block, 0, stream>>>(b.bytes, b.buf_bytes, b.descs, b.n_frames, b.out, b.results,
+                                                             d_need_hi, d_need_hi, CLX_INTERNAL_NEED_HIGH_ORDER);
+        (*launches)++;
+        if (fused) {
+            // The marked frames' planar samples -> interleaved, over every element of each: nothing the fast path wrote
+            // for them survives.  Gated like the 12-tap instance: exits at once when the fast path declined nothing.
+            e = launch_interleave(b.descs, b.n_frames, plan.max_frame_elems, b.out, b.conv, b.mode, stream, launches, b.mark,
+                                  d_generic);
+            if (e != cudaSuccess) return e;
+        }
     }
-    // Frames with an LPC order above 12 (non-subset streams) were only flagged by the 12-tap
-    // instance; the 32-tap instance picks them up.  It exits immediately when nothing was flagged.
-    decode_frames_kernel<32><<<grid, block, 0, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results,
-                                                         d_need_hi, d_need_hi, CLX_INTERNAL_NEED_HIGH_ORDER);
-    if (launches) *launches += 2;
-    if (fused) {
-        // The marked frames' planar samples -> interleaved, over every element of each: nothing the fast path wrote
-        // for them survives.  Gated like the 12-tap instance: exits at once when the fast path declined nothing.
-        e = launch_interleave(d_descs, n_frames, fused->max_frame_elems, d_out, fused->d_dst, fused->mode, stream, fused->d_mark,
-                              d_generic);
+    if (crc) {  // src/frame.rs:752-763, after the subframes
+        e = launch_crc16(b.bytes, b.descs, b.n_frames, b.results, stream, launches);
         if (e != cudaSuccess) return e;
-        if (launches) *launches += 1;
+    }
+    if (b.mode != CLX_OUT_PLANAR_I32 && !fused) {
+        e = launch_interleave(b.descs, b.n_frames, plan.max_frame_elems, b.out, b.conv, b.mode, stream, launches);
+        if (e != cudaSuccess) return e;
     }
     return cudaGetLastError();
 }

@@ -313,33 +313,6 @@ using SubIO = TmaIO<64>;
 using SubIO = DeviceIO<DEC_RQ, 3>;
 #endif
 
-// One trip of the recurrence for U consecutive samples.  v[0..TAPS) = history (oldest first),
-// v[TAPS+i] = sample i of this trip.  Terms that only involve history are summed first, the terms
-// with fresh samples last, most recent last — the serial chain per sample is one multiply-add,
-// the shift and the residual add.  ACC = long long is the reference's arithmetic verbatim; ACC = int
-// is the same recurrence in wrapping 32-bit arithmetic, bit-identical whenever
-// sum|coef| * max|sample| < 2^31 — which is re-checked against the samples actually produced.
-template <int TAPS, int U, typename ACC>
-__device__ __forceinline__ void seq_trip(int32_t (&v)[TAPS + U], const int32_t (&c)[TAPS], const int32_t* r, uint32_t shift) {
-    ACC part[U];
-#pragma unroll
-    for (int i = 0; i < U; i++) {
-        ACC acc = 0;
-#pragma unroll
-        for (int j = 0; j < TAPS; j++)
-            if (i + TAPS - 1 - j < TAPS) acc += (ACC)c[j] * (ACC)v[i + TAPS - 1 - j];
-        part[i] = acc;
-    }
-#pragma unroll
-    for (int i = 0; i < U; i++) {
-        ACC acc = part[i];
-#pragma unroll
-        for (int j = TAPS - 1; j >= 0; j--)
-            if (i + TAPS - 1 - j >= TAPS) acc += (ACC)c[j] * (ACC)v[i + TAPS - 1 - j];
-        v[TAPS + i] = (int32_t)(acc >> shift) + r[i];
-    }
-}
-
 // Where the samples of a tile row (= a lane = a subframe) go; shared memory, one per lane.  Rows 2p and 2p+1
 // are neighbouring channels of one frame when the batch has at least two channel slots — `ca` on the even
 // row is then the frame's stereo mode if the pair is its (channel 0, channel 1) — and two unrelated mono
@@ -387,9 +360,6 @@ __device__ __forceinline__ void il_store_row(const SeqRow& r, uint32_t g, const 
     if (g + 3 < r.bs) il_store<OM>(frame, e + 3 * nch, v.w);
 }
 
-__device__ __forceinline__ uint32_t seq_tile_word(uint32_t row, uint32_t col) {
-    return row * 32 + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3));
-}
 __device__ __forceinline__ void seq_store_vec(int32_t* out, uint32_t bs, bool vec, uint32_t g, const int4& v) {
     if (out == nullptr || g >= bs) return;
     if (vec && g + 4 <= bs) *reinterpret_cast<int4*>(out + g) = v;
@@ -561,7 +531,7 @@ __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint
             for (int j = TAPS - 1; j > 0; j--) h[j] = h[j - 1];
             h[0] = val;
             int32_t* fill = tile_ptr(fill_s);
-            fill[seq_tile_word(lane, t & 31)] = val;
+            fill[tile_word(lane, t & 31)] = val;
             if ((t & 31) == 31) seq_flush<true, OM>(fill, pr, t - 31, lane, any_wasted);
         }
     };
@@ -765,7 +735,7 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
             if (d.channel_assignment == 9) bits += (c == 0);
             else if (d.channel_assignment == 8 || d.channel_assignment == 10) bits += (c == 1);
             // valid streams keep |sample| <= 2^(bits-1); anything beyond is caught by the check below
-            narrow_ok = ((unsigned long long)absum << (bits - 1)) < (1ull << 31);
+            narrow_ok = i32_acc_exact(absum, bits);
             bit0 = (uint32_t)(d.byte_offset & 15) * 8;
             byte_len = d.byte_len;
         }
@@ -864,26 +834,30 @@ int g_exp_which = 3;
 int g_exp_dyn_smem = 0;  // extra dynamic shared memory per decode CTA: lowers occupancy (measurement only)
 #endif
 
-size_t seq_scratch_bytes(const CoopPlan& plan, uint32_t n_frames) {
+size_t seq_scratch_bytes(const Plan& plan, uint32_t n_frames) {
     const uint32_t n_warps = (n_frames + 31) / 32;
     const size_t b = (size_t)n_warps * 32 * plan.channels * sizeof(SeqParams);
     return ((b + 511) & ~(size_t)511) + 512;
 }
 
 cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
-                       int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, void* d_params,
-                       const CoopPlan& plan, cudaStream_t stream, int which, uint32_t mode) {
+                       int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, int* d_need_wide, void* d_params,
+                       const Plan& plan, uint32_t mode, cudaStream_t stream, uint64_t* launches) {
 #ifdef CLX_EXPERIMENT
-    which &= g_exp_which;
+    const int which = g_exp_which;
+#else
+    const int which = 3;
 #endif
     const uint32_t CH = plan.channels;
     uint32_t ch_log2 = 0;
     while ((1u << ch_log2) < CH) ch_log2++;
     const uint32_t n_warps = (n_frames + 31) / 32;
     SeqParams* params = reinterpret_cast<SeqParams*>(d_params);
-    if (which & 1)
+    if (which & 1) {
         index_frames_kernel<<<n_warps, 32, 0, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_results, params, CH,
                                                         d_need_generic);
+        (*launches)++;
+    }
     if (which & 2) {
         const uint32_t n_pwarps = n_warps * CH;
         dim3 g2((n_pwarps + DEC_WARPS - 1) / DEC_WARPS), b2(DEC_WARPS * 32);
@@ -892,10 +866,15 @@ cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_fra
 #else
         const size_t dyn = 0;
 #endif
-#define CLX_DEC(C, W, M) decode_subframes_kernel<C, W, M><<<g2, b2, dyn, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, params, CH, ch_log2, n_pwarps, d_need_generic, d_need_generic + 2)
-#define CLX_DEC4(M)                                                \
-    do {                                                           \
-        CLX_DEC(0, false, M); CLX_DEC(1, false, M);                \
+#define CLX_DEC(C, W, M)                                                                                                  \
+    do {                                                                                                                  \
+        decode_subframes_kernel<C, W, M><<<g2, b2, dyn, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, \
+                                                                  params, CH, ch_log2, n_pwarps, d_need_generic, d_need_wide); \
+        (*launches)++;                                                                                                    \
+    } while (0)
+#define CLX_DEC4(M)                                                      \
+    do {                                                                 \
+        CLX_DEC(0, false, M); CLX_DEC(1, false, M);                      \
         if (!plan.no_wide) { CLX_DEC(0, true, M); CLX_DEC(1, true, M); } \
     } while (0)
         if (mode == CLX_OUT_INTERLEAVED_I16) CLX_DEC4(CLX_OUT_INTERLEAVED_I16);

@@ -1,4 +1,6 @@
-// clx_lanes.h — the per-lane halves of the throughput path (clx_fused.cu).
+// clx_lanes.h — the per-lane halves of the throughput path (clx_fused.cu), and the small pieces of FLAC arithmetic
+// the decoders share: sign extension, byte swap, the fixed predictor rows, the i32-accumulator bound, the
+// staging tile's swizzle and the recurrence trip.
 //
 // FLAC gives no subframe lengths: channel n+1 starts at the bit where channel n ended (reference
 // src/frame.rs:702-742), so something has to walk channel n before channel n+1 can be touched.  The
@@ -102,8 +104,54 @@ CLX_HD uint32_t hd_bswap(uint32_t v) {
     return __builtin_bswap32(v);
 #endif
 }
-CLX_HD int32_t hd_sext(uint32_t v, uint32_t bits) {  // bits in [1, 32]
+CLX_HD int32_t hd_sext(uint32_t v, uint32_t bits) {  // bits in [1, 32]; src/subframe.rs:117-122
     return ((int32_t)(v << (32 - bits))) >> (32 - bits);
+}
+
+// ---------------------------------------------------------------------------------
+// Pieces of FLAC arithmetic the decoders share (clx_decode.cu, clx_coop.cu, clx_fused.cu)
+// ---------------------------------------------------------------------------------
+// Fixed predictor of `order` (0..4): rows {1}, {2,-1}, {3,-3,1}, {4,-6,4,-1} of src/subframe.rs:427-431, one signed
+// byte per coefficient; byte j multiplies s[t-1-j].
+CLX_HD uint32_t fixed_coefs_packed(uint32_t order) {
+    return order == 1 ? 0x00000001u : order == 2 ? 0x0000ff02u : order == 3 ? 0x0001fd03u : order == 4 ? 0xff04fa04u : 0u;
+}
+// The i32 accumulator is exact for a subframe of `bits`-bit samples (|sample| <= 2^(bits-1) in a valid stream) and
+// coefficients of sum |coef| = absum when no sum of products can leave the i32 range.
+CLX_HD bool i32_acc_exact(uint32_t absum, uint32_t bits) {
+    return ((unsigned long long)absum << (bits - 1)) < (1ull << 31);
+}
+// Shared-memory staging tile of 32 rows x 32 columns of i32: 16-byte groups XOR-swizzled by (row & 7), so that
+// both 16-byte stores of 8 lanes into 8 rows and row-wise 16-byte loads are free of bank conflicts.
+CLX_HD uint32_t tile_word(uint32_t row, uint32_t col) {
+    return row * 32 + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3));
+}
+// One trip of the recurrence for U consecutive samples.  v[0..TAPS) = history (oldest first), v[TAPS+i] = sample i of
+// this trip, r[i] its residual.  Terms that only involve history are summed first (they do not depend on this trip's
+// samples), the terms with fresh samples last, most recent last — the serial chain per sample is then one
+// multiply-add, the shift and the residual add.  ACC = long long is the reference's arithmetic verbatim (i64 products
+// and sum, src/subframe.rs:576-581); ACC = int is the same recurrence in wrapping 32-bit arithmetic, bit-identical
+// whenever no sum of products leaves the i32 range (see i32_acc_exact; the callers re-check it against the samples
+// actually produced).
+template <int TAPS, int U, typename ACC>
+CLX_HD void seq_trip(int32_t (&v)[TAPS + U], const int32_t (&c)[TAPS], const int32_t* r, uint32_t shift) {
+    ACC part[U];
+#pragma unroll
+    for (int i = 0; i < U; i++) {
+        ACC acc = 0;
+#pragma unroll
+        for (int j = 0; j < TAPS; j++)  // c[j] multiplies v[i + TAPS - 1 - j]; history only here
+            if (i + TAPS - 1 - j < TAPS) acc += (ACC)c[j] * (ACC)v[i + TAPS - 1 - j];
+        part[i] = acc;
+    }
+#pragma unroll
+    for (int i = 0; i < U; i++) {
+        ACC acc = part[i];
+#pragma unroll
+        for (int j = TAPS - 1; j >= 0; j--)  // fresh samples, oldest first
+            if (i + TAPS - 1 - j >= TAPS) acc += (ACC)c[j] * (ACC)v[i + TAPS - 1 - j];
+        v[TAPS + i] = (int32_t)(acc >> shift) + r[i];
+    }
 }
 
 enum : uint32_t { SEQ_SUBFRAME = 0, SEQ_PART = 1, SEQ_RUN = 2, SEQ_DONE = 3 };
@@ -482,9 +530,8 @@ struct IndexLane {
                 sp->coefs[j] = (int16_t)c;
                 absum += (uint32_t)(c < 0 ? -c : c);
             }
-        } else {  // rows of src/subframe.rs:427-431; coefs[0] multiplies s[t-1]
-            const uint32_t packed = order == 1 ? 0x00000001u : order == 2 ? 0x0000ff02u
-                                  : order == 3 ? 0x0001fd03u : order == 4 ? 0xff04fa04u : 0u;
+        } else {
+            const uint32_t packed = fixed_coefs_packed(order);
             for (uint32_t j = 0; j < order; j++) {
                 const int32_t c = (int32_t)(int8_t)(packed >> (8 * j));
                 sp->coefs[j] = (int16_t)c;

@@ -54,7 +54,8 @@ uint32_t output_elem_size(uint32_t mode) {
 }
 
 cudaError_t launch_interleave(const clx_frame_desc* d_descs, uint32_t n_frames, uint32_t max_frame_elems, const int32_t* d_planar,
-                              void* d_dst, uint32_t mode, cudaStream_t stream, const uint8_t* sel, const int* gate) {
+                              void* d_dst, uint32_t mode, cudaStream_t stream, uint64_t* launches, const uint8_t* sel,
+                              const int* gate) {
     if (n_frames == 0 || mode == CLX_OUT_PLANAR_I32) return cudaSuccess;
     const uint32_t tiles = (max_frame_elems + IL_TILE - 1) / IL_TILE;
     for (uint32_t f0 = 0; f0 < n_frames; f0 += 65535) {  // gridDim.y limit
@@ -68,6 +69,7 @@ cudaError_t launch_interleave(const clx_frame_desc* d_descs, uint32_t n_frames, 
         else
             interleave_kernel<4><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (uint8_t*)d_dst, s, gate);
     }
+    (*launches)++;  // one pass, however many grids its frames need
     return cudaGetLastError();
 }
 
@@ -80,9 +82,10 @@ mark_status_kernel(const clx_frame_result* __restrict__ results, uint32_t n_fram
 }
 
 cudaError_t launch_mark_status(const clx_frame_result* d_results, uint32_t n_frames, int32_t status, uint8_t* d_mark,
-                               const int* gate, cudaStream_t stream) {
+                               const int* gate, cudaStream_t stream, uint64_t* launches) {
     if (n_frames == 0) return cudaSuccess;
     mark_status_kernel<<<(n_frames + 255) / 256, 256, 0, stream>>>(d_results, n_frames, status, d_mark, gate);
+    (*launches)++;
     return cudaGetLastError();
 }
 

@@ -22,10 +22,11 @@ from . import _lib
 from ._lib import (OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT)
 from ._lib import (FrameDesc, FrameResult, OPT_NO_VERIFY_CRC, OPT_GENERIC_KERNEL_ONLY, OPT_WARP_PER_FRAME, OPT_LANE_PER_FRAME,
                    OPT_NO_GENERIC, OPT_NO_WIDE, FRAME_VARIABLE_BLOCKING, FRAME_CRC16_VERIFIED,
-                   OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24)
+                   OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24,
+                   OUT_CHANNELS_I32, OUT_CHANNELS_F32)
 
 __all__ = ["Error", "Block", "FrameReader", "FlacReader", "FlacReaderOptions", "StreamInfo", "Context", "DeviceBatch",
-           "parse_frame_header", "demux_frames", "open_stream", "ogg_frames", "mp4_frames", "status_str", "DESC_DTYPE", "RESULT_DTYPE"]
+           "parse_frame_header", "demux_frames", "open_stream", "ogg_frames", "mp4_frames", "status_str", "DESC_DTYPE", "RESULT_DTYPE", "load", "plan_columns"]
 
 # numpy views of the C structs (same layout; asserted below)
 DESC_DTYPE = np.dtype([
@@ -270,16 +271,19 @@ class Context:
     def host_free(self, arr: np.ndarray):
         self._L.clx_host_free(arr.ctypes.data)
 
-    def upload(self, data, descs: np.ndarray, out_elems: int, mode: int = OUT_PLANAR_I32) -> "DeviceBatch":
+    def upload(self, data, descs: np.ndarray, out_elems: int | None = None, mode: int = OUT_PLANAR_I32,
+               channels: int | None = None, channel_stride: int | None = None) -> "DeviceBatch":
         """A device-resident batch.  `mode`: the form its output is kept in, as for decode_frames (out_offset and
-        out_elems count samples in every mode)."""
-        return DeviceBatch(self, data, descs, out_elems, mode=mode)
+        out_elems count samples in every mode), or channels-first OUT_CHANNELS_I32 / _F32: a [channels,
+        channel_stride] buffer in which out_offset is each frame's column (out_elems omitted, or their product)."""
+        return DeviceBatch(self, data, descs, out_elems, mode=mode, channels=channels, channel_stride=channel_stride)
 
-    def adopt(self, device_ptr: int, nbytes: int, descs: np.ndarray, out_elems: int,
-              mode: int = OUT_PLANAR_I32) -> "DeviceBatch":
+    def adopt(self, device_ptr: int, nbytes: int, descs: np.ndarray, out_elems: int | None = None,
+              mode: int = OUT_PLANAR_I32, channels: int | None = None, channel_stride: int | None = None) -> "DeviceBatch":
         """A batch whose frame bytes already sit in this GPU's memory at `device_ptr` (e.g. a torch tensor's
         data_ptr() after the NCCL scatter of claxon_b200.shard.scatter_batch): copied device to device."""
-        return DeviceBatch(self, None, descs, out_elems, device_ptr=device_ptr, nbytes=nbytes, mode=mode)
+        return DeviceBatch(self, None, descs, out_elems, device_ptr=device_ptr, nbytes=nbytes, mode=mode,
+                           channels=channels, channel_stride=channel_stride)
 
 
 def _out_array(out_elems: int, mode: int) -> np.ndarray:
@@ -289,29 +293,50 @@ def _out_array(out_elems: int, mode: int) -> np.ndarray:
             np.empty(3 * n, dtype=np.uint8) if mode == OUT_INTERLEAVED_I24 else np.empty(n, dtype=np.int32))
 
 
+_CHANNEL_MODES = (OUT_CHANNELS_I32, OUT_CHANNELS_F32)
+
+
 class DeviceBatch:
     """clx_batch: frames resident in HBM; decode() launches the kernels only."""
 
-    def __init__(self, ctx: Context, data, descs: np.ndarray, out_elems: int, device_ptr: int | None = None,
-                 nbytes: int = 0, mode: int = OUT_PLANAR_I32):
+    def __init__(self, ctx: Context, data, descs: np.ndarray, out_elems: int | None, device_ptr: int | None = None,
+                 nbytes: int = 0, mode: int = OUT_PLANAR_I32, channels: int | None = None,
+                 channel_stride: int | None = None):
         self.ctx = ctx
         self.descs = np.ascontiguousarray(descs, dtype=DESC_DTYPE)
-        self.out_elems = int(out_elems)
         self.mode = int(mode)
-        h = C.c_void_p()
-        if device_ptr is None:
-            buf = _as_u8(data)
-            self.nbytes = int(buf.size)
-            _check(ctx._L.clx_batch_create_to(ctx._h, buf.ctypes.data, buf.size, self.descs.ctypes.data, self.descs.size,
-                                              self.out_elems, 0, self.mode, C.byref(h)), ctx)
+        self.channels = self.channel_stride = None
+        self._stream = None  # internal stream of the last decode()
+        # (a channel mode without its layout goes to clx_batch_create_to, which refuses it like any unknown mode)
+        if channels is not None or channel_stride is not None:
+            if self.mode not in _CHANNEL_MODES or channels is None or channel_stride is None:
+                raise ValueError("channels= and channel_stride= go together, with a channel mode")
+            self.channels, self.channel_stride = int(channels), int(channel_stride)
+            if out_elems is not None and int(out_elems) != self.channels * self.channel_stride:
+                raise ValueError("out_elems must equal channels * channel_stride")
+            out_elems = self.channels * self.channel_stride
+        if out_elems is None:
+            raise ValueError("out_elems is required")
+        self.out_elems = int(out_elems)
+        on_device = device_ptr is not None
+        if on_device:
+            ptr, self.nbytes = device_ptr, int(nbytes)
         else:
-            self.nbytes = int(nbytes)
-            _check(ctx._L.clx_batch_create_to(ctx._h, device_ptr, self.nbytes, self.descs.ctypes.data, self.descs.size,
-                                              self.out_elems, _lib.BATCH_BYTES_ON_DEVICE, self.mode, C.byref(h)), ctx)
+            buf = _as_u8(data)
+            ptr, self.nbytes = buf.ctypes.data, int(buf.size)
+        flags = _lib.BATCH_BYTES_ON_DEVICE if on_device else 0
+        h = C.c_void_p()
+        if self.channels is not None:
+            _check(ctx._L.clx_batch_create_channels(ctx._h, ptr, self.nbytes, self.descs.ctypes.data, self.descs.size,
+                                                    self.channels, self.channel_stride, flags, self.mode, C.byref(h)), ctx)
+        else:
+            _check(ctx._L.clx_batch_create_to(ctx._h, ptr, self.nbytes, self.descs.ctypes.data, self.descs.size,
+                                              self.out_elems, flags, self.mode, C.byref(h)), ctx)
         self._h = h
 
     def decode(self, stream: int = 0):
         _check(self.ctx._L.clx_batch_decode(self.ctx._h, self._h, stream), self.ctx)
+        self._stream = stream
 
     def sync(self):
         _check(self.ctx._L.clx_batch_sync(self.ctx._h, self._h), self.ctx)
@@ -322,12 +347,36 @@ class DeviceBatch:
         return float(ms.value)
 
     def read(self):
-        """Returns (out, results); `out` is in the batch's mode: int32, int16, or uint8 with 3 bytes per sample."""
-        out = _out_array(self.out_elems, self.mode)
+        """Returns (out, results); `out` is in the batch's mode: int32, int16, or uint8 with 3 bytes per sample; in a
+        channel mode an int32 / float32 array of shape (channels, channel_stride)."""
+        if self.channels is not None:
+            out = np.empty((self.channels, self.channel_stride),
+                           dtype=np.float32 if self.mode == OUT_CHANNELS_F32 else np.int32)
+        else:
+            out = _out_array(self.out_elems, self.mode)
         results = np.zeros(self.descs.size, dtype=RESULT_DTYPE)
         _check(self.ctx._L.clx_batch_read_to(self.ctx._h, self._h, out.ctypes.data, max(1, self.out_elems),
                                              results.ctypes.data), self.ctx)
         return out, results
+
+    def results(self):
+        """The per-frame results of the last decode (waits for it), without copying the samples."""
+        results = np.zeros(self.descs.size, dtype=RESULT_DTYPE)
+        _check(self.ctx._L.clx_batch_read_to(self.ctx._h, self._h, None, 0, results.ctypes.data), self.ctx)
+        return results
+
+    def tensor(self):
+        """A zero-copy torch CUDA tensor [channels, channel_stride] (float32 or int32) over the batch's output, for the
+        channel modes.  It keeps the batch alive and shows whatever the batch's latest decode wrote; torch's current
+        stream is made to wait for the last decode() first, so it may be read on that stream without a sync.
+        (close() frees the memory under it.)"""
+        import torch
+        if self.channels is None:
+            raise ValueError("tensor() needs a batch in a channel mode")
+        if self._stream is not None:
+            ptr = self.ctx._L.clx_ctx_stream(self.ctx._h, self._stream)
+            torch.cuda.current_stream().wait_stream(torch.cuda.ExternalStream(ptr))
+        return torch.as_tensor(_CudaArray(self), device="cuda")
 
     @property
     def device_out_ptr(self) -> int:
@@ -343,6 +392,17 @@ class DeviceBatch:
             self.close()
         except Exception:
             pass
+
+
+class _CudaArray:
+    """__cuda_array_interface__ of a channel-mode batch's output; holds the batch while a tensor views it."""
+
+    def __init__(self, batch: DeviceBatch):
+        self.batch = batch
+        self.__cuda_array_interface__ = {
+            "shape": (batch.channels, batch.channel_stride),
+            "typestr": "<f4" if batch.mode == OUT_CHANNELS_F32 else "<i4",
+            "data": (batch.device_out_ptr, False), "strides": None, "version": 2}
 
 
 _default_ctx: Context | None = None
@@ -596,3 +656,93 @@ class FlacReader:
 
     def into_inner(self):
         return self._frames.into_inner() if self._frames is not None else None
+
+
+# ---------------------------------------------------------------------------
+# FLAC files -> torch tensors
+# ---------------------------------------------------------------------------
+
+def plan_columns(files_descs: list[np.ndarray]):
+    """Column layout of several files' frames in one channels-first batch.  Returns (descs, starts, lengths, rows,
+    stride): the files' descriptors concatenated with out_offset = each frame's column (its file's start plus the
+    block sizes of the frames before it), each file's first column (a multiple of 4), each file's sample count per
+    channel, the largest channel count, and the row length (the end of the last file rounded up to a multiple of 4)."""
+    starts, lengths, parts = [], [], []
+    at, rows = 0, 0
+    for d in files_descs:
+        d = np.array(d, dtype=DESC_DTYPE)
+        bs = d["block_size"].astype(np.uint64)
+        d["out_offset"] = at + np.concatenate([[0], np.cumsum(bs)[:-1]]).astype(np.uint64) if d.size else bs
+        n = int(bs.sum())
+        starts.append(at)
+        lengths.append(n)
+        parts.append(d)
+        rows = max(rows, int(d["n_channels"].max()) if d.size else 0)
+        at = (at + n + 3) & ~3
+    descs = np.concatenate(parts) if parts else np.zeros(0, dtype=DESC_DTYPE)
+    return descs, starts, lengths, rows, at
+
+
+def _read_source(src) -> np.ndarray:
+    if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)):
+        return _as_u8(src)
+    with open(src, "rb") as f:
+        return np.frombuffer(f.read(), dtype=np.uint8)
+
+
+def load(src, dtype=None, ctx: Context | None = None, threads: int = 0):
+    """FLAC file(s) -> (tensor [channels, samples], sample_rate) on the GPU, channels first like torchaudio.load.
+
+    `src`: a path or the file's bytes, or a list of them (then a list of results).  `dtype`: torch.float32 (the
+    default: samples * 2^-(bits_per_sample - 1), in [-1, 1)) or torch.int32.  Every file is demuxed on `threads` host
+    threads (0 = all) and all of them are decoded in one device-resident batch; each result is a view of one tensor.
+    Raises what FlacReader would: the metadata error, a frame-header error where demuxing stopped, or the first frame
+    that failed (naming the file); ValueError for a frame whose channel count differs from STREAMINFO's."""
+    import torch
+    dtype = torch.float32 if dtype is None else dtype
+    if dtype not in (torch.float32, torch.int32):
+        raise ValueError("dtype must be torch.float32 or torch.int32")
+    many = isinstance(src, (list, tuple))
+    bufs = [_read_source(s) for s in (src if many else [src])]
+    infos, file_descs, bases, open_ends = [], [], [], []
+    base = 0
+    for i, buf in enumerate(bufs):
+        si, first = open_stream(buf)
+        descs, _, _, stop = demux_frames(buf, first, threads=threads)
+        # OK: the last frame's end could not be confirmed (damage, or bytes after it); its decode gives the verdict
+        if stop not in (OK, EOF):
+            raise Error(stop, f"file {i}")
+        open_ends.append(stop == OK and descs.size > 0)
+        if descs.size and (descs["n_channels"] != si.channels).any():
+            raise ValueError(f"file {i}: a frame's channel count differs from STREAMINFO's ({si.channels})")
+        descs["byte_offset"] += np.uint64(base)
+        infos.append(si)
+        file_descs.append(descs)
+        bases.append(base)
+        base += buf.size
+    descs, starts, lengths, rows, stride = plan_columns(file_descs)
+    # (the batch's buffer reads 0 wherever no frame wrote, so one copy of it fills every element)
+    out = (torch.empty if descs.size else torch.zeros)((max(rows, 1), stride), dtype=dtype, device="cuda")
+    if descs.size:
+        ctx = ctx or default_context()
+        mode = OUT_CHANNELS_F32 if dtype == torch.float32 else OUT_CHANNELS_I32
+        dev = ctx.upload(np.concatenate(bufs), descs, mode=mode, channels=rows, channel_stride=stride)
+        try:
+            dev.decode(0)
+            res = dev.results()
+            bad = np.nonzero(res["status"] != OK)[0]
+            if bad.size:
+                f = int(np.searchsorted(np.cumsum([d.size for d in file_descs]), bad[0], side="right"))
+                raise Error(int(res["status"][bad[0]]), f"file {f}")
+            ends = np.cumsum([d.size for d in file_descs]) - 1
+            for i, last in enumerate(ends):
+                if open_ends[i] and res["consumed"][last] < descs["byte_len"][last]:  # what follows the last frame
+                    st, _ = parse_frame_header(bufs[i], int(descs["byte_offset"][last]) - bases[i] + int(res["consumed"][last]))
+                    if st != EOF:
+                        raise Error(st, f"file {i}")
+            out.copy_(dev.tensor())
+            torch.cuda.current_stream().synchronize()  # the copy has completed: nothing of the batch is needed
+        finally:
+            dev.close()
+    views = [(out[:si.channels, s:s + n], si.sample_rate) for si, s, n in zip(infos, starts, lengths)]
+    return views if many else views[0]

@@ -50,6 +50,7 @@ OPT_NO_WIDE = 32
 OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT = 1, 2
 BATCH_BYTES_ON_DEVICE = 1
 OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24 = 0, 1, 2, 3
+OUT_CHANNELS_I32, OUT_CHANNELS_F32 = 4, 5
 FRAME_VARIABLE_BLOCKING = 1
 FRAME_CRC16_VERIFIED = 2
 
@@ -80,6 +81,8 @@ SYMBOLS = {
     "clx_batch_create": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _sz, C.POINTER(_vp)]),
     "clx_batch_create_ex": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _sz, C.c_uint32, C.POINTER(_vp)]),
     "clx_batch_create_to": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _sz, C.c_uint32, C.c_uint32, C.POINTER(_vp)]),
+    "clx_batch_create_channels": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, C.c_uint32, _sz, C.c_uint32, C.c_uint32,
+                                            C.POINTER(_vp)]),
     "clx_batch_decode": (C.c_int, [_vp, _vp, C.c_uint32]),
     "clx_batch_sync": (C.c_int, [_vp, _vp]),
     "clx_batch_read": (C.c_int, [_vp, _vp, _vp, _sz, _vp]),

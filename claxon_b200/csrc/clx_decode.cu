@@ -684,10 +684,19 @@ decode_frames_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes,
 cudaError_t launch_decode(const DecodeBuffers& b, const Plan& plan, bool crc, cudaStream_t stream, uint64_t* launches) {
     if (b.n_frames == 0) return cudaSuccess;
     const bool fast = plan.path != Path::Generic;
-    // The lane-per-frame decode pass writes interleaved I32 / I16 itself when the caller keeps the frames to convert
-    // after the generic kernel (`mark`); every other path, and I24, decodes to planar and converts all frames at the end.
+    // The lane-per-frame decode pass writes interleaved I32 / I16 and the channels modes itself when the caller keeps the
+    // frames to convert after the generic kernel (`mark`); every other path, and I24, decodes to planar and converts all
+    // frames at the end.
+    const bool channels = b.mode == CLX_OUT_CHANNELS_I32 || b.mode == CLX_OUT_CHANNELS_F32;
     const bool fused = plan.path == Path::LanePerFrame && b.mark != nullptr &&
-                       (b.mode == CLX_OUT_INTERLEAVED_I32 || b.mode == CLX_OUT_INTERLEAVED_I16);
+                       (b.mode == CLX_OUT_INTERLEAVED_I32 || b.mode == CLX_OUT_INTERLEAVED_I16 || channels);
+    // planar -> the batch's mode, for the frames in `sel` (all if null) unless *gate == 0
+    auto convert = [&](const uint8_t* sel, const int* gate) {
+        return channels ? launch_channels(b.descs, b.n_frames, plan.max_frame_elems, b.out, b.conv, b.cols, b.stride, b.mode,
+                                          stream, launches, sel, gate)
+                        : launch_interleave(b.descs, b.n_frames, plan.max_frame_elems, b.out, b.conv, b.mode, stream,
+                                            launches, sel, gate);
+    };
     int* d_generic = b.flags;        // set by a fast path: some frames need the generic kernel
     int* d_need_hi = b.flags + 1;    // set by the 12-tap generic instance: some frames need 32 taps
     int* d_need_wide = b.flags + 2;  // set by the lane-per-frame decode pass: some frames need the i64 second chance
@@ -695,7 +704,8 @@ cudaError_t launch_decode(const DecodeBuffers& b, const Plan& plan, bool crc, cu
     if (e != cudaSuccess) return e;
     if (plan.path == Path::LanePerFrame)
         e = launch_seq(b.bytes, b.buf_bytes, b.descs, b.n_frames, fused ? static_cast<int32_t*>(b.conv) : b.out, b.results,
-                       d_generic, d_need_wide, b.params, plan, fused ? b.mode : (uint32_t)CLX_OUT_PLANAR_I32, stream, launches);
+                       d_generic, d_need_wide, b.params, plan, fused ? b.mode : (uint32_t)CLX_OUT_PLANAR_I32, b.cols, b.stride,
+                       stream, launches);
     else if (plan.path == Path::WarpPerFrame)
         e = launch_warp_per_frame(b.bytes, b.buf_bytes, b.descs, b.n_frames, b.out, b.results, d_generic, b.params, plan,
                                   stream, launches);
@@ -718,10 +728,9 @@ cudaError_t launch_decode(const DecodeBuffers& b, const Plan& plan, bool crc, cu
                                                              d_need_hi, d_need_hi, CLX_INTERNAL_NEED_HIGH_ORDER);
         (*launches)++;
         if (fused) {
-            // The marked frames' planar samples -> interleaved, over every element of each: nothing the fast path wrote
-            // for them survives.  Gated like the 12-tap instance: exits at once when the fast path declined nothing.
-            e = launch_interleave(b.descs, b.n_frames, plan.max_frame_elems, b.out, b.conv, b.mode, stream, launches, b.mark,
-                                  d_generic);
+            // The marked frames' planar samples -> the batch's mode, over every element of each: nothing the fast path
+            // wrote for them survives.  Gated like the 12-tap instance: exits at once when the fast path declined nothing.
+            e = convert(b.mark, d_generic);
             if (e != cudaSuccess) return e;
         }
     }
@@ -730,7 +739,7 @@ cudaError_t launch_decode(const DecodeBuffers& b, const Plan& plan, bool crc, cu
         if (e != cudaSuccess) return e;
     }
     if (b.mode != CLX_OUT_PLANAR_I32 && !fused) {
-        e = launch_interleave(b.descs, b.n_frames, plan.max_frame_elems, b.out, b.conv, b.mode, stream, launches);
+        e = convert(nullptr, nullptr);
         if (e != cudaSuccess) return e;
     }
     return cudaGetLastError();

@@ -17,7 +17,8 @@
 //      of a frame together, which turns the wasted-bits shift (src/subframe.rs:216-225) and the
 //      inter-channel decorrelation (src/frame.rs:319-389) into a few operations per PAIR of 16-byte
 //      vectors, and writes planar i32 as whole 128-byte lines — or, for a device-resident batch in an
-//      interleaved i32 / i16 mode, the interleaved samples themselves (DESIGN.md §3.1).
+//      interleaved i32 / i16 mode, the interleaved samples themselves, and in a channels-first i32 / f32 mode
+//      the rows of a [channels, stride] buffer (DESIGN.md §3.1).
 //
 // HBM traffic per frame: its bytes once for the decode, the bytes of all channels but the last once more
 // for the index pass, 224 bytes of parameters per subframe, and the planar i32 output once.
@@ -322,12 +323,25 @@ using SubIO = DeviceIO<DEC_RQ, 3>;
 // little-endian integer of 4 / 2 bytes.  In the interleaved instances `out` is the FRAME's first element (the same
 // for all its rows), bit 0 of `meta` says that this address is 16-byte aligned, and bits 24-27 / 28-31 hold the
 // frame's channel count and the row's channel.
+// CLX_OUT_CHANNELS_I32 / _F32 write a channels-first buffer: `out` is the row's first element, `out + c * stride +
+// column`, and the flush takes the planar branches (rows are independent addresses).  In F32, bits 24-29 of `meta`
+// hold the frame header's bits_per_sample, whose power of two scales the row.
 struct __align__(16) SeqRow {
     int32_t* out;   // subframe's first output element (nullptr: idle row)
     uint32_t bs;    // block size
     uint32_t meta;  // bit 0: 16-byte stores allowed; bits 8-15: wasted bits; bits 16-19 (even rows): 8 left/side,
                     // 9 side/right, 10 mid/side, 0 independent
 };
+
+__host__ __device__ constexpr bool is_interleaved(int om) { return om == CLX_OUT_INTERLEAVED_I32 || om == CLX_OUT_INTERLEAVED_I16; }
+__host__ __device__ constexpr bool is_channels(int om) { return om == CLX_OUT_CHANNELS_I32 || om == CLX_OUT_CHANNELS_F32; }
+
+// ---- channels-first f32 output: (float)s * 2^-(bps-1), rounded to nearest even, stored as the float's bits ----
+__device__ __forceinline__ float f32_scale(uint32_t bps) { return __int_as_float((int)(128u - bps) << 23); }
+__device__ __forceinline__ int4 to_f32(const int4& v, float s) {
+    return make_int4(__float_as_int(__fmul_rn(__int2float_rn(v.x), s)), __float_as_int(__fmul_rn(__int2float_rn(v.y), s)),
+                     __float_as_int(__fmul_rn(__int2float_rn(v.z), s)), __float_as_int(__fmul_rn(__int2float_rn(v.w), s)));
+}
 
 // ---- interleaved output ----
 template <int OM>
@@ -389,7 +403,8 @@ __device__ __forceinline__ void mid_side(int32_t& a, int32_t& b) {
 // 16-byte vectors of a row pair (rows 2p, 2p+1), so each store instruction of the warp covers four whole
 // 128-byte lines — scattering the lanes over more rows costs the load/store unit a wavefront per line.
 // CHECKED = false is for tiles wholly inside every active row with 16-byte stores allowed everywhere.
-// Interleaved (OM != planar): a quarter holds whole frames (CH <= 8 channel slots, a frame's channels are CH
+// Channels-first: the planar stores, at the rows' own addresses; F32 converts after decorrelation.
+// Interleaved: a quarter holds whole frames (CH <= 8 channel slots, a frame's channels are CH
 // consecutive rows), and a lane writes what it holds: four interleaved pairs when its rows are a stereo frame's two
 // channels and the frame base is 16-byte aligned, else element by element.
 template <bool CHECKED, int OM = CLX_OUT_PLANAR_I32>
@@ -412,7 +427,11 @@ __device__ __forceinline__ void seq_flush_quarter(const int32_t* tile, const Seq
         a.x = (int32_t)((uint32_t)a.x + (uint32_t)b.x); a.y = (int32_t)((uint32_t)a.y + (uint32_t)b.y);
         a.z = (int32_t)((uint32_t)a.z + (uint32_t)b.z); a.w = (int32_t)((uint32_t)a.w + (uint32_t)b.w);
     }
-    if constexpr (OM != CLX_OUT_PLANAR_I32) {
+    if constexpr (OM == CLX_OUT_CHANNELS_F32) {
+        a = to_f32(a, f32_scale((i0.meta >> 24) & 63u));
+        b = to_f32(b, f32_scale((i1.meta >> 24) & 63u));
+    }
+    if constexpr (is_interleaved(OM)) {
         // (an idle row's meta has no channel count: never a pair)
         const bool pair = ((i0.meta >> 24) & 15u) == 2 && (i0.meta >> 28) == 0;
         if (pair && (!CHECKED || ((i0.meta & 1u) != 0 && g + 4 <= i0.bs))) {
@@ -452,11 +471,12 @@ __device__ __forceinline__ void sts128(uint32_t addr, int32_t a, int32_t b, int3
 // inside every row.
 //   tile_s: shared address of the tile to write out;  outp_s: shared address of the warp's 32 row pointers;
 //   lc0 / lc1: the lane's constant offsets into the tile for rows (2p, 2p+1) of its quarter (see decode_rows).
-// Interleaved (OM != planar, only for batches of stereo frames: CH == 2): rows (2p, 2p+1) are one frame's left and
-// right channel, and the lane's four samples of each are four interleaved pairs at the frame's element 2g.
+// Interleaved (only for batches of stereo frames: CH == 2): rows (2p, 2p+1) are one frame's left and right channel,
+// and the lane's four samples of each are four interleaved pairs at the frame's element 2g.
+// Channels-first: the planar stores at the rows' own addresses; in F32 every row of the warp has the scale `fs`.
 template <int UCA, int OM = CLX_OUT_PLANAR_I32>
 __device__ __forceinline__ void flush_quarter_fast(uint32_t tile_s, uint32_t outp_s, uint32_t g0, uint32_t quarter, uint32_t lane,
-                                                   uint32_t lc0, uint32_t lc1) {
+                                                   uint32_t lc0, uint32_t lc1, float fs = 0.f) {
     const uint32_t a0 = tile_s + quarter * 1024u + lc0;
     const int4 a = lds128(a0);
     const int4 b = lds128(a0 + lc1);
@@ -469,6 +489,10 @@ __device__ __forceinline__ void flush_quarter_fast(uint32_t tile_s, uint32_t out
         ob = make_int4(a.x - hx, a.y - hy, a.z - hz, a.w - hw);
     }
     const uint32_t off = (g0 + (lane & 7u) * 4u) * 4u;  // bytes
+    if constexpr (OM == CLX_OUT_CHANNELS_F32) {
+        oa = to_f32(oa, fs);
+        ob = to_f32(ob, fs);
+    }
     if constexpr (OM == CLX_OUT_INTERLEAVED_I16) {
         il_store_pairs<OM>(reinterpret_cast<uint8_t*>(p0) + off, oa, ob);  // element 2g, 2 bytes each: byte 4g
     } else if constexpr (OM == CLX_OUT_INTERLEAVED_I32) {
@@ -484,11 +508,12 @@ __device__ __forceinline__ void flush_quarter_fast(uint32_t tile_s, uint32_t out
 // end), so the 32x32 tile fills row by row in step and is flushed as whole lines.
 //   tile_s: shared address of the warp's two tiles (8 KB, 8 KB-aligned: the other tile is `addr ^ 4096`).
 //   FMODE: 0 = general flush; 1 / 2 = flush_quarter_fast applies, without stereo decorrelation / mid-side.
+//   fs: channels-first F32 with FMODE != 0, the warp's one scale.
 template <int TAPS, int U, typename ACC, int FMODE, int OM>
 __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint32_t order, uint32_t shift,
                                             const SeqParams* __restrict__ sp, bool active, int32_t* tile, uint32_t tile_s,
                                             const SeqRow* pr, uint32_t outp_s, uint32_t lane, bool all_vec,
-                                            bool any_wasted, int32_t& smin, int32_t& smax) {
+                                            bool any_wasted, int32_t& smin, int32_t& smax, float fs) {
     int32_t c[TAPS], h[TAPS];  // c[j] multiplies s[t-1-j]; h[j] = s[t-1-j]
 #pragma unroll
     for (int j = 0; j < TAPS; j++) {
@@ -590,7 +615,7 @@ __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint
         auto after = [&](uint32_t t) {
             if (have_drain) {  // a tile inside [head_end, bulk_end) lies inside every active row
                 const uint32_t g0 = (t & ~31u) - 32, quarter = (t >> 3) & 3;
-                if (FMODE != 0) flush_quarter_fast<FMODE == 2 ? 10 : 0, OM>(fill_s ^ 4096u, outp_s, g0, quarter, lane, lc0, lc1);
+                if (FMODE != 0) flush_quarter_fast<FMODE == 2 ? 10 : 0, OM>(fill_s ^ 4096u, outp_s, g0, quarter, lane, lc0, lc1, fs);
                 else if (all_vec) seq_flush_quarter<false, OM>(tile_ptr(fill_s ^ 4096u), pr, g0, quarter, lane, any_wasted);
                 else seq_flush_quarter<true, OM>(tile_ptr(fill_s ^ 4096u), pr, g0, quarter, lane, any_wasted);
             }
@@ -678,15 +703,17 @@ __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint
 // below): the same rows once more with the reference's i64 arithmetic only.  It looks at nothing unless the first
 // pass raised `need_wide`.
 //
-// OM: the output mode (see SeqRow).  The interleaved instances write a frame's samples straight into the caller's
-// interleaved buffer `out`, after wasted bits and decorrelation as the planar flush applies them; the planar
-// instance is the one every other path shares.
+// OM: the output mode (see SeqRow).  The interleaved and channels instances write a frame's samples straight into the
+// batch's buffer `out`, after wasted bits and decorrelation as the planar flush applies them; the planar instance is
+// the one every other path shares.  `cols` / `stride` (channels instances only; the others ignore them): the frame's
+// column, per frame in the order of `descs`, and the row length of the channels buffer.
 template <int GROUP, bool WIDE, int OM = CLX_OUT_PLANAR_I32>
 __global__ void __launch_bounds__(DEC_WARPS * 32)
 decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, const clx_frame_desc* __restrict__ descs,
                         uint32_t n_frames, int32_t* __restrict__ out, clx_frame_result* __restrict__ results,
                         const SeqParams* __restrict__ params, uint32_t CH, uint32_t ch_log2, uint32_t n_pwarps,
-                        int* __restrict__ need_generic, int* __restrict__ need_wide) {
+                        int* __restrict__ need_generic, int* __restrict__ need_wide, const uint64_t* __restrict__ cols,
+                        uint64_t stride) {
     __shared__ __align__(8192) int32_t s_tile[DEC_WARPS][2 * 32 * 32];  // two tiles: one fills while the other drains
     __shared__ SeqRow s_rows[DEC_WARPS][32];
     __shared__ __align__(16) int32_t* s_outp[DEC_WARPS][32];
@@ -726,7 +753,10 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
             absum = sp->absum;
             ca = d.channel_assignment >= 8 ? d.channel_assignment : 0u;
             if constexpr (OM == CLX_OUT_PLANAR_I32) sub = out + d.out_offset + (size_t)c * bs;
-            else {  // the frame's first interleaved element
+            else if constexpr (is_channels(OM)) {  // the row's first element
+                sub = out + c * stride + cols[f];
+                if (OM == CLX_OUT_CHANNELS_F32) il_meta = (uint32_t)d.bits_per_sample << 24;
+            } else {  // the frame's first interleaved element
                 sub = reinterpret_cast<int32_t*>(reinterpret_cast<uint8_t*>(out) +
                                                  d.out_offset * (OM == CLX_OUT_INTERLEAVED_I16 ? 2u : 4u));
                 il_meta = ((uint32_t)d.n_channels << 24) | (c << 28);
@@ -764,14 +794,22 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
     // (with one channel slot per frame, rows 2p and 2p+1 are unrelated frames: mode 0)
     const uint32_t pair_ca = CH >= 2 ? __shfl_sync(0xffffffffu, ca, lane & ~1u) : 0u;
     const uint32_t ca0 = __shfl_sync(0xffffffffu, pair_ca, 0);
-    // (interleaved: only stereo batches, whose row pairs are the two channels of one frame)
-    const bool fast_flush = (OM == CLX_OUT_PLANAR_I32 || CH == 2) &&
+    // (interleaved: only stereo batches, whose row pairs are the two channels of one frame; channels-first F32: one
+    // bits_per_sample, hence one scale, for the whole warp)
+    float fs = 0.f;
+    bool one_scale = true;
+    if constexpr (OM == CLX_OUT_CHANNELS_F32) {
+        const uint32_t bps0 = __shfl_sync(0xffffffffu, il_meta >> 24, 0);
+        one_scale = __all_sync(0xffffffffu, (il_meta >> 24) == bps0);
+        fs = f32_scale(bps0);
+    }
+    const bool fast_flush = (!is_interleaved(OM) || CH == 2) && one_scale &&
                             __all_sync(0xffffffffu, active && vec_own && wasted == 0 && pair_ca == ca0);
     const int fmode = !fast_flush ? 0 : ca0 == 0 ? 1 : ca0 == 10 ? 2 : 0;
     int32_t smin = 0, smax = 0;
     const uint32_t tile_s = (uint32_t)__cvta_generic_to_shared(tile);
     const uint32_t outp_s = (uint32_t)__cvta_generic_to_shared(&s_outp[warp][0]);
-#define CLX_ROWS(T, UU, A, F) decode_rows<T, UU, A, F, OM>(L, bs, order, shift, sp, active, tile, tile_s, pr, outp_s, lane, all_vec, any_wasted, smin, smax)
+#define CLX_ROWS(T, UU, A, F) decode_rows<T, UU, A, F, OM>(L, bs, order, shift, sp, active, tile, tile_s, pr, outp_s, lane, all_vec, any_wasted, smin, smax, fs)
     // straight-line flush variants only where they pay: the i32-accumulator bodies (16-bit audio).  The i64 bodies are
     // what mixed batches run, several per SM at a time; there one body (12 taps, also for warps that would do with
     // 8) beats two that evict each other from the instruction cache.
@@ -842,7 +880,8 @@ size_t seq_scratch_bytes(const Plan& plan, uint32_t n_frames) {
 
 cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
                        int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, int* d_need_wide, void* d_params,
-                       const Plan& plan, uint32_t mode, cudaStream_t stream, uint64_t* launches) {
+                       const Plan& plan, uint32_t mode, const uint64_t* d_cols, uint64_t stride, cudaStream_t stream,
+                       uint64_t* launches) {
 #ifdef CLX_EXPERIMENT
     const int which = g_exp_which;
 #else
@@ -869,7 +908,8 @@ cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_fra
 #define CLX_DEC(C, W, M)                                                                                                  \
     do {                                                                                                                  \
         decode_subframes_kernel<C, W, M><<<g2, b2, dyn, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, \
-                                                                  params, CH, ch_log2, n_pwarps, d_need_generic, d_need_wide); \
+                                                                  params, CH, ch_log2, n_pwarps, d_need_generic, d_need_wide, \
+                                                                  d_cols, stride);                                        \
         (*launches)++;                                                                                                    \
     } while (0)
 #define CLX_DEC4(M)                                                      \
@@ -879,6 +919,8 @@ cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_fra
     } while (0)
         if (mode == CLX_OUT_INTERLEAVED_I16) CLX_DEC4(CLX_OUT_INTERLEAVED_I16);
         else if (mode == CLX_OUT_INTERLEAVED_I32) CLX_DEC4(CLX_OUT_INTERLEAVED_I32);
+        else if (mode == CLX_OUT_CHANNELS_I32) CLX_DEC4(CLX_OUT_CHANNELS_I32);
+        else if (mode == CLX_OUT_CHANNELS_F32) CLX_DEC4(CLX_OUT_CHANNELS_F32);
         else CLX_DEC4(CLX_OUT_PLANAR_I32);
 #undef CLX_DEC4
 #undef CLX_DEC

@@ -36,9 +36,11 @@ size_t seq_scratch_bytes(const Plan& plan, uint32_t n_frames);
 
 // The device buffers of one decode.  `bytes`: 256-byte aligned, buf_bytes = allocated size, a multiple of 64 with at
 // least 128 bytes of slack after the last frame.  `flags`: four device ints of scratch.  `out`: planar i32 (the
-// output in mode CLX_OUT_PLANAR_I32, else the generic kernel's scratch); `conv`: the output of an interleaved mode.
-// `mark` (one byte per frame, optional): given, a LanePerFrame decode to interleaved I32 / I16 writes `conv` itself;
-// `mark` then records which frames the generic kernel takes over, and only those are converted after it.
+// output in mode CLX_OUT_PLANAR_I32, else the generic kernel's scratch); `conv`: the output of an interleaved or
+// channels mode.  `mark` (one byte per frame, optional): given, a LanePerFrame decode to interleaved I32 / I16 or to a
+// channels mode writes `conv` itself; `mark` then records which frames the generic kernel takes over, and only those
+// are converted after it.  Channels modes only: `cols`, the column of each frame in the order of `descs` (whose
+// out_offset is then the frame's place in the planar scratch `out`), and `stride`, the row length of `conv`.
 struct DecodeBuffers {
     const uint8_t* bytes;
     uint64_t buf_bytes;
@@ -51,6 +53,8 @@ struct DecodeBuffers {
     uint32_t mode;
     void* conv;
     uint8_t* mark;
+    const uint64_t* cols;
+    uint64_t stride;
 };
 // The whole launch sequence of one decode on `stream`: the plan's kernels, the device CRC-16 when `crc`, the
 // conversion to an interleaved mode.  Every kernel launched adds one to *launches.
@@ -60,10 +64,12 @@ cudaError_t launch_decode(const DecodeBuffers& b, const Plan& plan, bool crc, cu
 cudaError_t launch_warp_per_frame(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
                                   int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, void* d_params,
                                   const Plan& plan, cudaStream_t stream, uint64_t* launches);
-// `mode`: the output mode the decode pass writes (planar, or interleaved I32 / I16 into `d_out`).
+// `mode`: the output mode the decode pass writes (planar, or interleaved I32 / I16 or channels I32 / F32 into `d_out`;
+// `d_cols` / `stride` as in DecodeBuffers).
 cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
                        int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, int* d_need_wide, void* d_params,
-                       const Plan& plan, uint32_t mode, cudaStream_t stream, uint64_t* launches);
+                       const Plan& plan, uint32_t mode, const uint64_t* d_cols, uint64_t stride, cudaStream_t stream,
+                       uint64_t* launches);
 // clx_crc.cu: frame CRC-16 of every frame that decoded (over the length the decode found), on the device
 cudaError_t crc16_init();  // once per context, on its device
 cudaError_t launch_crc16(const uint8_t* d_bytes, const clx_frame_desc* d_descs, uint32_t n_frames, clx_frame_result* d_results,
@@ -74,6 +80,11 @@ uint32_t output_elem_size(uint32_t mode);
 cudaError_t launch_interleave(const clx_frame_desc* d_descs, uint32_t n_frames, uint32_t max_frame_elems, const int32_t* d_planar,
                               void* d_dst, uint32_t mode, cudaStream_t stream, uint64_t* launches, const uint8_t* sel = nullptr,
                               const int* gate = nullptr);
+// planar i32 -> channels-first i32 / f32 (CLX_OUT_CHANNELS_*): row c of frame f at d_dst + c * stride + d_cols[f].
+// `sel` / `gate` as for launch_interleave.
+cudaError_t launch_channels(const clx_frame_desc* d_descs, uint32_t n_frames, uint32_t max_frame_elems, const int32_t* d_planar,
+                            void* d_dst, const uint64_t* d_cols, uint64_t stride, uint32_t mode, cudaStream_t stream,
+                            uint64_t* launches, const uint8_t* sel = nullptr, const int* gate = nullptr);
 // mark[f] = (results[f].status == status) for every frame, unless *gate == 0 (then nothing is written).
 cudaError_t launch_mark_status(const clx_frame_result* d_results, uint32_t n_frames, int32_t status, uint8_t* d_mark,
                                const int* gate, cudaStream_t stream, uint64_t* launches);

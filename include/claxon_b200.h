@@ -223,6 +223,26 @@ int clx_batch_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const
  * with CLX_OUT_PLANAR_I32. */
 int clx_batch_create_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
                         size_t n_frames, size_t out_elems, uint32_t batch_flags, uint32_t mode, clx_batch** out);
+/* Channels-first output for device-resident batches: one [n_channels, channel_stride] buffer of 4-byte elements, the
+ * layout PyTorch audio code uses (one row per channel, time along the row).  In these modes descs[i].out_offset is
+ * the frame's COLUMN: row c < descs[i].n_channels gets that channel's block_size samples at columns [out_offset,
+ * out_offset + block_size), after wasted bits and decorrelation as in the planar layout.  Rows a frame does not have
+ * are left alone.  The buffer is zeroed once when the batch is created, so elements that no frame covers read 0 and
+ * stay 0.  A failed frame's region is fully overwritten with what the planar layout holds for it, converted.
+ * CLX_OUT_CHANNELS_F32 stores (float)s * 2^-(bits_per_sample - 1), bits_per_sample being the frame header's value:
+ * the int-to-float conversion rounds to nearest even and the multiply is exact, so every sample of a valid stream of
+ * at most 24 bits maps exactly into [-1, 1).
+ * CLX_ERR_INVALID_ARGUMENT for: n_channels 0 or above 8, channel_stride 0, n_channels * channel_stride * 4
+ * overflowing, a frame with more channels than n_channels or with out_offset + block_size > channel_stride, in F32 a
+ * frame with bits_per_sample above 24, a mode other than the two below, and every byte-range condition of the other
+ * create calls.  clx_batch_read_to copies min(out_elems, n_channels * channel_stride) elements; clx_batch_read refuses.
+ * On the lane-per-frame path the decode kernel writes the rows itself; every other path decodes to a planar scratch
+ * buffer and converts inside the batch's graph.  (clx_batch_create_to and clx_decode_frames_to refuse these modes.) */
+#define CLX_OUT_CHANNELS_I32 4u /* out[c * channel_stride + t]: sample t of channel c, i32 */
+#define CLX_OUT_CHANNELS_F32 5u /* the same as float: (float)s * 2^-(bits_per_sample - 1) */
+int clx_batch_create_channels(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
+                              size_t n_frames, uint32_t n_channels, size_t channel_stride, uint32_t batch_flags,
+                              uint32_t mode, clx_batch** out);
 int clx_batch_decode(clx_ctx* ctx, clx_batch* b, uint32_t stream_index); /* async on an internal stream */
 int clx_batch_sync(clx_ctx* ctx, clx_batch* b);
 /* Planar batches only (CLX_ERR_INVALID_ARGUMENT for any other mode). */

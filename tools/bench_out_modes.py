@@ -1,12 +1,14 @@
-"""Steady-state throughput of device-resident batches per output mode (planar i32 / interleaved i32 / i16).
+"""Steady-state throughput of device-resident batches per output mode (planar i32 / interleaved i32 / i16 /
+channels-first i32 / f32).
 
 The method of bench.py's steady state: `--units` resident batches of one workload, every one decoded once before
 timing, then `--steps` steps round-robin over `--streams` streams through Context.run_steps (CUDA events).  The
 modes are timed alternately in one process, `--rounds` times each; the median and the spread (max - min over the
 median) are reported per mode, with the output bytes per sample, whether one batch per mode equals the generator's
-PCM byte for byte, and the card's name, power limit and SM clock read in the same run.
+PCM byte for byte, and the card's name, power limit and SM clock read in the same run.  A channels-first batch holds
+one unit as rows of its samples per channel, the frames' columns packed back to back.
 
-    python tools/bench_out_modes.py                      # C2 (i32 / i16 / planar), C3 (i32 / planar), C4 (i16 / planar)
+    python tools/bench_out_modes.py                      # C2, C3, C4: planar, their interleaved modes, channels i32 / f32
     python tools/bench_out_modes.py --workloads c2 --steps 1000
 """
 from __future__ import annotations
@@ -24,13 +26,31 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import claxon_b200 as cb  # noqa: E402
 from claxon_b200 import synth  # noqa: E402
 
-ESIZE = {cb.OUT_PLANAR_I32: 4, cb.OUT_INTERLEAVED_I32: 4, cb.OUT_INTERLEAVED_I16: 2}
-NAMES = {cb.OUT_PLANAR_I32: "planar_i32", cb.OUT_INTERLEAVED_I32: "interleaved_i32", cb.OUT_INTERLEAVED_I16: "interleaved_i16"}
+CH_I32, CH_F32 = cb.OUT_CHANNELS_I32, cb.OUT_CHANNELS_F32
+ESIZE = {cb.OUT_PLANAR_I32: 4, cb.OUT_INTERLEAVED_I32: 4, cb.OUT_INTERLEAVED_I16: 2, CH_I32: 4, CH_F32: 4}
+NAMES = {cb.OUT_PLANAR_I32: "planar_i32", cb.OUT_INTERLEAVED_I32: "interleaved_i32", cb.OUT_INTERLEAVED_I16: "interleaved_i16",
+         CH_I32: "channels_i32", CH_F32: "channels_f32"}
 PLAN = {  # workload -> (frames per unit, units, modes)
-    "c2": (1024, 128, (cb.OUT_PLANAR_I32, cb.OUT_INTERLEAVED_I16, cb.OUT_INTERLEAVED_I32)),
-    "c3": (8192, 8, (cb.OUT_PLANAR_I32, cb.OUT_INTERLEAVED_I32)),
-    "c4": (1100, 128, (cb.OUT_PLANAR_I32, cb.OUT_INTERLEAVED_I16)),
+    "c2": (1024, 128, (cb.OUT_PLANAR_I32, cb.OUT_INTERLEAVED_I16, cb.OUT_INTERLEAVED_I32, CH_I32, CH_F32)),
+    "c3": (8192, 8, (cb.OUT_PLANAR_I32, cb.OUT_INTERLEAVED_I32, CH_I32, CH_F32)),
+    "c4": (1100, 128, (cb.OUT_PLANAR_I32, cb.OUT_INTERLEAVED_I16, CH_I32, CH_F32)),
 }
+
+
+def channels_layout(descs):
+    """(descs with out_offset = column, rows, stride): the unit's frames back to back along each row."""
+    d = descs.copy()
+    bs = d["block_size"].astype(np.uint64)
+    d["out_offset"] = np.concatenate([[0], np.cumsum(bs)[:-1]]).astype(np.uint64)
+    return d, int(d["n_channels"].max()), int(bs.sum())
+
+
+def upload(ctx, b, descs, out_elems, mode):
+    if mode in (CH_I32, CH_F32):
+        d, rows, stride = channels_layout(descs)
+        assert rows * stride == out_elems  # one shape per unit: every element is a sample
+        return ctx.upload(b.data, d, mode=mode, channels=rows, channel_stride=stride)
+    return ctx.upload(b.data, descs, out_elems, mode=mode)
 
 
 def gpu_info():
@@ -47,6 +67,12 @@ def expected_bytes(b, descs, out_elems, mode):
     """The generator's PCM in the mode's layout (planar i32, or interleaved little-endian elements)."""
     if mode == cb.OUT_PLANAR_I32:
         return b.pcm[:out_elems].astype("<i4").tobytes()
+    if mode in (CH_I32, CH_F32):
+        rows = np.concatenate([b.pcm[int(b.pcm_offsets[i]):int(b.pcm_offsets[i + 1])].reshape(int(descs[i]["n_channels"]), -1)
+                               for i in range(b.n_frames)], axis=1)
+        if mode == CH_F32:
+            rows = rows.astype(np.float32) * np.float32(2.0 ** -(int(descs[0]["bits_per_sample"]) - 1))  # one width per workload
+        return rows.astype("<f4" if mode == CH_F32 else "<i4").tobytes()
     parts = []
     for i in range(b.n_frames):
         nch = int(descs[i]["n_channels"])
@@ -67,7 +93,7 @@ def run_workload(ctx, name, units, steps, streams, rounds, warmup):
         descs, out_elems = cb.descs_from_offsets(b.data, b.frame_offsets[:-1], b.frame_lengths)
         assert out_elems == b.n_samples  # frames back to back: every output byte is a sample
         for m in modes:
-            batches[m].append(ctx.upload(b.data, descs, out_elems, mode=m))
+            batches[m].append(upload(ctx, b, descs, out_elems, m))
         samples += b.n_samples
         if u == 0:
             first = (b, descs, out_elems)
@@ -77,7 +103,7 @@ def run_workload(ctx, name, units, steps, streams, rounds, warmup):
         dev = batches[m][0]
         dev.decode(0)
         out, res = dev.read()
-        got = out.view(np.uint8)[:out_elems * ESIZE[m]].tobytes()
+        got = out.reshape(-1).view(np.uint8)[:out_elems * ESIZE[m]].tobytes()
         exact[NAMES[m]] = bool((res["status"] == 0).all()) and got == expected_bytes(b, descs, out_elems, m)
     for m in modes:  # every batch once, every graph warm
         ctx.run_steps(batches[m], max(warmup, units), streams)

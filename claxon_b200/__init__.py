@@ -20,13 +20,14 @@ import numpy as np
 
 from . import _lib
 from ._lib import (OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT)
-from ._lib import (FrameDesc, FrameResult, OPT_NO_VERIFY_CRC, OPT_GENERIC_KERNEL_ONLY, OPT_WARP_PER_FRAME, OPT_LANE_PER_FRAME,
+from ._lib import (FrameDesc, FrameResult, FrameWindow, OPT_NO_VERIFY_CRC, OPT_GENERIC_KERNEL_ONLY, OPT_WARP_PER_FRAME, OPT_LANE_PER_FRAME,
                    OPT_NO_GENERIC, OPT_NO_WIDE, FRAME_VARIABLE_BLOCKING, FRAME_CRC16_VERIFIED,
                    OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24,
                    OUT_CHANNELS_I32, OUT_CHANNELS_F32)
 
 __all__ = ["Error", "Block", "FrameReader", "FlacReader", "FlacReaderOptions", "StreamInfo", "Context", "DeviceBatch",
-           "parse_frame_header", "demux_frames", "open_stream", "ogg_frames", "mp4_frames", "status_str", "DESC_DTYPE", "RESULT_DTYPE", "load", "plan_columns"]
+           "parse_frame_header", "demux_frames", "open_stream", "ogg_frames", "mp4_frames", "status_str", "DESC_DTYPE", "RESULT_DTYPE", "load", "plan_columns",
+           "WINDOW_DTYPE", "index", "FlacIndex", "IndexedFile", "load_crops", "plan_range", "frame_starts"]
 
 # numpy views of the C structs (same layout; asserted below)
 DESC_DTYPE = np.dtype([
@@ -34,7 +35,9 @@ DESC_DTYPE = np.dtype([
     ("n_channels", "u1"), ("channel_assignment", "u1"), ("bits_per_sample", "u1"), ("flags", "u1"),
     ("sample_rate", "<u4"), ("number", "<u8"), ("out_offset", "<u8")], align=True)
 RESULT_DTYPE = np.dtype([("status", "<i4"), ("consumed", "<u4")], align=True)
+WINDOW_DTYPE = np.dtype([("row", "<u4"), ("first", "<u4"), ("count", "<u4"), ("reserved", "<u4")], align=True)
 assert DESC_DTYPE.itemsize == C.sizeof(FrameDesc) and RESULT_DTYPE.itemsize == C.sizeof(FrameResult)
+assert WINDOW_DTYPE.itemsize == C.sizeof(FrameWindow)
 
 KIND_NONE, KIND_IO, KIND_FORMAT, KIND_UNSUPPORTED, KIND_LIBRARY = range(5)
 OK, EOF = 0, 1
@@ -272,18 +275,24 @@ class Context:
         self._L.clx_host_free(arr.ctypes.data)
 
     def upload(self, data, descs: np.ndarray, out_elems: int | None = None, mode: int = OUT_PLANAR_I32,
-               channels: int | None = None, channel_stride: int | None = None) -> "DeviceBatch":
+               channels: int | None = None, channel_stride: int | None = None,
+               windows: np.ndarray | None = None) -> "DeviceBatch":
         """A device-resident batch.  `mode`: the form its output is kept in, as for decode_frames (out_offset and
         out_elems count samples in every mode), or channels-first OUT_CHANNELS_I32 / _F32: a [channels,
-        channel_stride] buffer in which out_offset is each frame's column (out_elems omitted, or their product)."""
-        return DeviceBatch(self, data, descs, out_elems, mode=mode, channels=channels, channel_stride=channel_stride)
+        channel_stride] buffer in which out_offset is each frame's column (out_elems omitted, or their product).
+        `windows` (channel modes; WINDOW_DTYPE, one per frame): frame i stores only samples [first, first + count)
+        of each channel c, on row `row + c`, from column out_offset on (clx_batch_create_windows); `channels` is
+        then the number of rows and has no cap of 8."""
+        return DeviceBatch(self, data, descs, out_elems, mode=mode, channels=channels, channel_stride=channel_stride,
+                           windows=windows)
 
     def adopt(self, device_ptr: int, nbytes: int, descs: np.ndarray, out_elems: int | None = None,
-              mode: int = OUT_PLANAR_I32, channels: int | None = None, channel_stride: int | None = None) -> "DeviceBatch":
+              mode: int = OUT_PLANAR_I32, channels: int | None = None, channel_stride: int | None = None,
+              windows: np.ndarray | None = None) -> "DeviceBatch":
         """A batch whose frame bytes already sit in this GPU's memory at `device_ptr` (e.g. a torch tensor's
         data_ptr() after the NCCL scatter of claxon_b200.shard.scatter_batch): copied device to device."""
         return DeviceBatch(self, None, descs, out_elems, device_ptr=device_ptr, nbytes=nbytes, mode=mode,
-                           channels=channels, channel_stride=channel_stride)
+                           channels=channels, channel_stride=channel_stride, windows=windows)
 
 
 def _out_array(out_elems: int, mode: int) -> np.ndarray:
@@ -301,7 +310,7 @@ class DeviceBatch:
 
     def __init__(self, ctx: Context, data, descs: np.ndarray, out_elems: int | None, device_ptr: int | None = None,
                  nbytes: int = 0, mode: int = OUT_PLANAR_I32, channels: int | None = None,
-                 channel_stride: int | None = None):
+                 channel_stride: int | None = None, windows: np.ndarray | None = None):
         self.ctx = ctx
         self.descs = np.ascontiguousarray(descs, dtype=DESC_DTYPE)
         self.mode = int(mode)
@@ -315,6 +324,13 @@ class DeviceBatch:
             if out_elems is not None and int(out_elems) != self.channels * self.channel_stride:
                 raise ValueError("out_elems must equal channels * channel_stride")
             out_elems = self.channels * self.channel_stride
+        if windows is not None:
+            if self.channels is None:
+                raise ValueError("windows= needs a channel mode with channels= and channel_stride=")
+            windows = np.ascontiguousarray(windows, dtype=WINDOW_DTYPE)
+            if windows.size != self.descs.size:
+                raise ValueError("one window per frame")
+        self.windows = windows
         if out_elems is None:
             raise ValueError("out_elems is required")
         self.out_elems = int(out_elems)
@@ -326,7 +342,11 @@ class DeviceBatch:
             ptr, self.nbytes = buf.ctypes.data, int(buf.size)
         flags = _lib.BATCH_BYTES_ON_DEVICE if on_device else 0
         h = C.c_void_p()
-        if self.channels is not None:
+        if windows is not None:
+            _check(ctx._L.clx_batch_create_windows(ctx._h, ptr, self.nbytes, self.descs.ctypes.data, windows.ctypes.data,
+                                                   self.descs.size, self.channels, self.channel_stride, flags, self.mode,
+                                                   C.byref(h)), ctx)
+        elif self.channels is not None:
             _check(ctx._L.clx_batch_create_channels(ctx._h, ptr, self.nbytes, self.descs.ctypes.data, self.descs.size,
                                                     self.channels, self.channel_stride, flags, self.mode, C.byref(h)), ctx)
         else:
@@ -662,6 +682,33 @@ class FlacReader:
 # FLAC files -> torch tensors
 # ---------------------------------------------------------------------------
 
+def frame_starts(descs: np.ndarray) -> np.ndarray:
+    """Each frame's first sample (int64): the running sum of the block sizes before it, in stream order."""
+    bs = descs["block_size"].astype(np.int64)
+    return np.concatenate([[0], np.cumsum(bs)[:-1]]).astype(np.int64) if bs.size else bs
+
+
+def plan_range(descs: np.ndarray, lo: int, hi: int, column: int = 0, row: int = 0, starts: np.ndarray | None = None):
+    """The frames of one stream that overlap its samples [lo, hi), and where they go.  Returns (idx, windows, cols):
+    the indices of those frames in `descs` (consecutive, in stream order), their windows (WINDOW_DTYPE: `row`, and
+    the first sample and count of each frame inside the range) and each window's column, so that sample lo of the
+    stream lands at column `column`.  `starts`: frame_starts(descs), if already known.  An empty range (or one past
+    the end) has no frames."""
+    if starts is None:
+        starts = frame_starts(descs)
+    bs = descs["block_size"].astype(np.int64)
+    i0 = int(np.searchsorted(starts + bs, lo, side="right"))  # the first frame that ends after lo
+    i1 = int(np.searchsorted(starts, hi, side="left")) if hi > lo else i0  # the frames that start before hi
+    idx = np.arange(i0, max(i0, i1), dtype=np.int64)
+    s0, b = starts[idx], bs[idx]
+    first = np.maximum(lo - s0, 0)
+    count = np.minimum(s0 + b, hi) - s0 - first
+    windows = np.zeros(idx.size, dtype=WINDOW_DTYPE)
+    windows["row"], windows["first"], windows["count"] = row, first, count
+    cols = (column + s0 + first - lo).astype(np.uint64)
+    return idx, windows, cols
+
+
 def plan_columns(files_descs: list[np.ndarray]):
     """Column layout of several files' frames in one channels-first batch.  Returns (descs, starts, lengths, rows,
     stride): the files' descriptors concatenated with out_offset = each frame's column (its file's start plus the
@@ -671,9 +718,10 @@ def plan_columns(files_descs: list[np.ndarray]):
     at, rows = 0, 0
     for d in files_descs:
         d = np.array(d, dtype=DESC_DTYPE)
-        bs = d["block_size"].astype(np.uint64)
-        d["out_offset"] = at + np.concatenate([[0], np.cumsum(bs)[:-1]]).astype(np.uint64) if d.size else bs
-        n = int(bs.sum())
+        n = int(d["block_size"].astype(np.int64).sum())
+        idx, _, cols = plan_range(d, 0, n, column=at)  # the whole file: every frame, full windows
+        d = d[idx]
+        d["out_offset"] = cols
         starts.append(at)
         lengths.append(n)
         parts.append(d)
@@ -683,6 +731,32 @@ def plan_columns(files_descs: list[np.ndarray]):
     return descs, starts, lengths, rows, at
 
 
+@dataclass
+class IndexedFile:
+    """One stream of a FlacIndex: its bytes, STREAMINFO, frame descriptors (byte_offset into `data`), each frame's
+    first sample, its length in samples per channel, and whether the end of its last frame was confirmed by the
+    demuxer (False: the decode of that frame gives the verdict on what follows it, as in FlacReader)."""
+    data: np.ndarray
+    info: StreamInfo
+    descs: np.ndarray
+    starts: np.ndarray
+    length: int
+    end_confirmed: bool
+
+
+class FlacIndex:
+    """Frame indexes of FLAC streams, demuxed once: what load_crops() plans excerpts from."""
+
+    def __init__(self, files: list[IndexedFile]):
+        self.files = files
+
+    def __len__(self) -> int:
+        return len(self.files)
+
+    def __getitem__(self, i: int) -> IndexedFile:
+        return self.files[i]
+
+
 def _read_source(src) -> np.ndarray:
     if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)):
         return _as_u8(src)
@@ -690,59 +764,161 @@ def _read_source(src) -> np.ndarray:
         return np.frombuffer(f.read(), dtype=np.uint8)
 
 
-def load(src, dtype=None, ctx: Context | None = None, threads: int = 0):
-    """FLAC file(s) -> (tensor [channels, samples], sample_rate) on the GPU, channels first like torchaudio.load.
+def _map_source(src) -> np.ndarray:
+    """A path as a read-only np.memmap (an empty file as an empty array); bytes as they are."""
+    if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)):
+        return _as_u8(src)
+    import os
+    if os.path.getsize(src) == 0:
+        return np.zeros(0, dtype=np.uint8)
+    return np.memmap(src, dtype=np.uint8, mode="r")
 
-    `src`: a path or the file's bytes, or a list of them (then a list of results).  `dtype`: torch.float32 (the
-    default: samples * 2^-(bits_per_sample - 1), in [-1, 1)) or torch.int32.  Every file is demuxed on `threads` host
-    threads (0 = all) and all of them are decoded in one device-resident batch; each result is a view of one tensor.
-    Raises what FlacReader would: the metadata error, a frame-header error where demuxing stopped, or the first frame
-    that failed (naming the file); ValueError for a frame whose channel count differs from STREAMINFO's."""
+
+def _index_one(buf: np.ndarray, i: int, threads: int) -> IndexedFile:
+    si, first = open_stream(buf)
+    descs, _, _, stop = demux_frames(buf, first, threads=threads)
+    # OK: the last frame's end could not be confirmed (damage, or bytes after it); its decode gives the verdict
+    if stop not in (OK, EOF):
+        raise Error(stop, f"file {i}")
+    if descs.size and (descs["n_channels"] != si.channels).any():
+        raise ValueError(f"file {i}: a frame's channel count differs from STREAMINFO's ({si.channels})")
+    starts = frame_starts(descs)
+    n = int(starts[-1]) + int(descs["block_size"][-1]) if descs.size else 0
+    return IndexedFile(buf, si, descs, starts, n, not (stop == OK and descs.size > 0))
+
+
+def index(src, threads: int = 0) -> FlacIndex:
+    """Opens and demuxes FLAC stream(s) once: `src` is a path or the file's bytes, or a list of them (paths are
+    memory-mapped).  Raises what load() raises at demux time: the metadata error, a frame-header error where
+    demuxing stopped, or ValueError for a frame whose channel count differs from STREAMINFO's."""
+    many = isinstance(src, (list, tuple))
+    return FlacIndex([_index_one(_map_source(s), i, threads) for i, s in enumerate(src if many else [src])])
+
+
+def _torch_dtype(dtype):
     import torch
     dtype = torch.float32 if dtype is None else dtype
     if dtype not in (torch.float32, torch.int32):
         raise ValueError("dtype must be torch.float32 or torch.int32")
+    return dtype
+
+
+def _decode_excerpts(idx: FlacIndex, excerpts, rows: int, stride: int, out, ctx: Context | None, where):
+    """Decodes excerpts of indexed files in one windowed batch into `out`, a torch tensor viewing [rows, stride].
+    `excerpts`: (file, lo, hi, column, row) per excerpt: samples [lo, hi) of the file go to row `row` + c from
+    column `column` on.  Only the frames overlapping an excerpt are gathered, uploaded and decoded.  where(k) names
+    excerpt k in errors."""
+    import torch
+    chunks, parts, wins, owner, at = [], [], [], [], 0
+    for k, (fi, lo, hi, column, row) in enumerate(excerpts):
+        f = idx.files[fi]
+        sel, w, cols = plan_range(f.descs, lo, hi, column=column, row=row, starts=f.starts)
+        if not sel.size:
+            continue
+        d = f.descs[sel]
+        b0 = int(d["byte_offset"][0])
+        b1 = int(d["byte_offset"][-1]) + int(d["byte_len"][-1])
+        chunks.append(f.data[b0:b1])
+        d["byte_offset"] = d["byte_offset"] - np.uint64(b0) + np.uint64(at)
+        d["out_offset"] = cols
+        parts.append(d)
+        wins.append(w)
+        owner.append(np.full(sel.size, k, np.int64))
+        at += b1 - b0
+    if not parts:
+        out.zero_()
+        return
+    descs, windows, owner = np.concatenate(parts), np.concatenate(wins), np.concatenate(owner)
+    ctx = ctx or default_context()
+    mode = OUT_CHANNELS_F32 if out.dtype == torch.float32 else OUT_CHANNELS_I32
+    dev = ctx.upload(np.concatenate(chunks), descs, mode=mode, channels=rows, channel_stride=stride, windows=windows)
+    try:
+        dev.decode(0)
+        res = dev.results()
+        bad = np.nonzero(res["status"] != OK)[0]
+        if bad.size:
+            raise Error(int(res["status"][bad[0]]), where(int(owner[bad[0]])))
+        # an excerpt that contains a file's unconfirmed last frame: what follows that frame
+        for j in np.nonzero(np.r_[owner[1:] != owner[:-1], True])[0]:
+            k = int(owner[j])
+            f = idx.files[excerpts[k][0]]
+            last = f.descs[-1]
+            if f.end_confirmed or excerpts[k][2] <= int(f.starts[-1]):
+                continue
+            if res["consumed"][j] < last["byte_len"]:
+                st, _ = parse_frame_header(f.data, int(last["byte_offset"]) + int(res["consumed"][j]))
+                if st != EOF:
+                    raise Error(st, where(k))
+        out.copy_(dev.tensor())
+        torch.cuda.current_stream().synchronize()  # the copy has completed: nothing of the batch is needed
+    finally:
+        dev.close()
+
+
+def load(src, dtype=None, ctx: Context | None = None, threads: int = 0, frame_offset: int = 0, num_frames: int = -1):
+    """FLAC file(s) -> (tensor [channels, samples], sample_rate) on the GPU, channels first like torchaudio.load.
+
+    `src`: a path or the file's bytes, or a list of them (then a list of results).  `dtype`: torch.float32 (the
+    default: samples * 2^-(bits_per_sample - 1), in [-1, 1)) or torch.int32.  `frame_offset` / `num_frames` as in
+    torchaudio: each file gives its samples [frame_offset, frame_offset + num_frames), cut at its end (num_frames -1:
+    to the end), so [C_i, min(num_frames, N_i - frame_offset)]; only the frames that overlap that range are decoded.
+    Every file is demuxed on `threads` host threads (0 = all) and all of them are decoded in one device-resident
+    batch; each result is a view of one tensor.  Raises what FlacReader would: the metadata error, a frame-header error
+    where demuxing stopped, or the first decoded frame that failed (naming the file); ValueError for a frame whose
+    channel count differs from STREAMINFO's, and for frame_offset < 0 or past a file's end or num_frames < -1."""
+    import torch
+    dtype = _torch_dtype(dtype)
+    if frame_offset < 0 or num_frames < -1:
+        raise ValueError("frame_offset must be >= 0 and num_frames >= -1")
     many = isinstance(src, (list, tuple))
-    bufs = [_read_source(s) for s in (src if many else [src])]
-    infos, file_descs, bases, open_ends = [], [], [], []
-    base = 0
-    for i, buf in enumerate(bufs):
-        si, first = open_stream(buf)
-        descs, _, _, stop = demux_frames(buf, first, threads=threads)
-        # OK: the last frame's end could not be confirmed (damage, or bytes after it); its decode gives the verdict
-        if stop not in (OK, EOF):
-            raise Error(stop, f"file {i}")
-        open_ends.append(stop == OK and descs.size > 0)
-        if descs.size and (descs["n_channels"] != si.channels).any():
-            raise ValueError(f"file {i}: a frame's channel count differs from STREAMINFO's ({si.channels})")
-        descs["byte_offset"] += np.uint64(base)
-        infos.append(si)
-        file_descs.append(descs)
-        bases.append(base)
-        base += buf.size
-    descs, starts, lengths, rows, stride = plan_columns(file_descs)
+    idx = FlacIndex([_index_one(_read_source(s), i, threads) for i, s in enumerate(src if many else [src])])
+    excerpts, spans, at, rows = [], [], 0, 0
+    for i, f in enumerate(idx.files):
+        if frame_offset > f.length:
+            raise ValueError(f"file {i}: frame_offset {frame_offset} is past its end ({f.length} samples)")
+        hi = f.length if num_frames < 0 else min(f.length, frame_offset + num_frames)
+        excerpts.append((i, frame_offset, hi, at, 0))
+        spans.append((at, hi - frame_offset))
+        rows = max(rows, f.info.channels if f.descs.size else 0)
+        at = (at + hi - frame_offset + 3) & ~3
     # (the batch's buffer reads 0 wherever no frame wrote, so one copy of it fills every element)
-    out = (torch.empty if descs.size else torch.zeros)((max(rows, 1), stride), dtype=dtype, device="cuda")
-    if descs.size:
-        ctx = ctx or default_context()
-        mode = OUT_CHANNELS_F32 if dtype == torch.float32 else OUT_CHANNELS_I32
-        dev = ctx.upload(np.concatenate(bufs), descs, mode=mode, channels=rows, channel_stride=stride)
-        try:
-            dev.decode(0)
-            res = dev.results()
-            bad = np.nonzero(res["status"] != OK)[0]
-            if bad.size:
-                f = int(np.searchsorted(np.cumsum([d.size for d in file_descs]), bad[0], side="right"))
-                raise Error(int(res["status"][bad[0]]), f"file {f}")
-            ends = np.cumsum([d.size for d in file_descs]) - 1
-            for i, last in enumerate(ends):
-                if open_ends[i] and res["consumed"][last] < descs["byte_len"][last]:  # what follows the last frame
-                    st, _ = parse_frame_header(bufs[i], int(descs["byte_offset"][last]) - bases[i] + int(res["consumed"][last]))
-                    if st != EOF:
-                        raise Error(st, f"file {i}")
-            out.copy_(dev.tensor())
-            torch.cuda.current_stream().synchronize()  # the copy has completed: nothing of the batch is needed
-        finally:
-            dev.close()
-    views = [(out[:si.channels, s:s + n], si.sample_rate) for si, s, n in zip(infos, starts, lengths)]
+    out = torch.empty((max(rows, 1), at), dtype=dtype, device="cuda")
+    _decode_excerpts(idx, excerpts, max(rows, 1), at, out, ctx, lambda k: f"file {k}")
+    views = [(out[:f.info.channels, s:s + n], f.info.sample_rate) for f, (s, n) in zip(idx.files, spans)]
     return views if many else views[0]
+
+
+def load_crops(index: FlacIndex, files, offsets, num_frames: int, dtype=None, ctx: Context | None = None):
+    """Excerpts of indexed FLAC files as one [B, C, num_frames] CUDA tensor, the batch a training loader wants.
+
+    Excerpt b is samples [offsets[b], offsets[b] + num_frames) of file files[b]; C is the largest channel count among
+    the chosen files.  Columns past a file's end, and rows a file does not have, read 0.  Returns (tensor, lengths):
+    lengths[b] = min(num_frames, N - offsets[b]) (a torch.int64 CPU tensor).  `dtype`: torch.float32 (the default, the
+    rule of load()) or torch.int32.  Only the frames that overlap an excerpt are gathered into one host buffer,
+    uploaded and decoded, in one batch whose rows are copied into the tensor once.  So errors of frames outside every
+    excerpt are not reported: raises Error(status, "file i, crop b") for the first failed frame inside an excerpt, or
+    for what follows a file's last frame (load()'s trailing-bytes check) when an excerpt contains that frame; ValueError
+    for an offset < 0 or past the file's end, num_frames < 1, a file index out of range, or another dtype."""
+    import torch
+    dtype = _torch_dtype(dtype)
+    files = [int(f) for f in np.asarray(files).reshape(-1)]
+    offsets = [int(o) for o in np.asarray(offsets).reshape(-1)]
+    num_frames = int(num_frames)
+    if len(files) != len(offsets):
+        raise ValueError("files and offsets must have the same length")
+    if num_frames < 1:
+        raise ValueError("num_frames must be >= 1")
+    for b, (fi, o) in enumerate(zip(files, offsets)):
+        if not 0 <= fi < len(index):
+            raise ValueError(f"crop {b}: file index {fi} out of range")
+        if not 0 <= o <= index[fi].length:
+            raise ValueError(f"crop {b}: offset {o} outside file {fi} ({index[fi].length} samples)")
+    B = len(files)
+    C_ = max([index[fi].info.channels for fi in files], default=1)
+    out = torch.empty((B, C_, num_frames), dtype=dtype, device="cuda")
+    excerpts = [(fi, o, min(o + num_frames, index[fi].length), 0, b * C_) for b, (fi, o) in enumerate(zip(files, offsets))]
+    lengths = torch.tensor([hi - lo for _, lo, hi, _, _ in excerpts], dtype=torch.int64)
+    if B:
+        _decode_excerpts(index, excerpts, B * C_, num_frames, out.view(B * C_, num_frames), ctx,
+                         lambda k: f"file {files[k]}, crop {k}")
+    return out, lengths

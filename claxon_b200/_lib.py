@@ -34,12 +34,16 @@ class StreamInfoC(C.Structure):
     ]
 
 
+class FrameWindow(C.Structure):
+    _fields_ = [("row", C.c_uint32), ("first", C.c_uint32), ("count", C.c_uint32), ("reserved", C.c_uint32)]
+
+
 class Options(C.Structure):
     _fields_ = [("device", C.c_int32), ("flags", C.c_uint32), ("n_streams", C.c_uint32),
                 ("host_threads", C.c_uint32)]
 
 
-assert C.sizeof(FrameDesc) == 40 and C.sizeof(FrameResult) == 8
+assert C.sizeof(FrameDesc) == 40 and C.sizeof(FrameResult) == 8 and C.sizeof(FrameWindow) == 16
 
 OPT_NO_VERIFY_CRC = 1
 OPT_GENERIC_KERNEL_ONLY = 2
@@ -83,6 +87,8 @@ SYMBOLS = {
     "clx_batch_create_to": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _sz, C.c_uint32, C.c_uint32, C.POINTER(_vp)]),
     "clx_batch_create_channels": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, C.c_uint32, _sz, C.c_uint32, C.c_uint32,
                                             C.POINTER(_vp)]),
+    "clx_batch_create_windows": (C.c_int, [_vp, _u8p, _sz, _vp, _vp, _sz, C.c_uint32, _sz, C.c_uint32, C.c_uint32,
+                                           C.POINTER(_vp)]),
     "clx_batch_decode": (C.c_int, [_vp, _vp, C.c_uint32]),
     "clx_batch_sync": (C.c_int, [_vp, _vp]),
     "clx_batch_read": (C.c_int, [_vp, _vp, _vp, _sz, _vp]),

@@ -142,11 +142,13 @@ struct clx_batch {
     // I24, decodes to d_out and converts all frames inside the graph (see clx::launch_decode).
     // Channels modes: d_conv holds out_elems = rows * stride elements, and the device descriptors' out_offset is the
     // frame's place in the planar scratch d_out (frames packed back to back, 4-element aligned); d_cols holds each
-    // frame's column, in the device order.
+    // frame's window start on row 0 (row base * stride + column), and d_wins its window (first | count << 16; full windows
+    // for clx_batch_create_channels), both in the device order.
     uint32_t mode = CLX_OUT_PLANAR_I32;
     void* d_conv = nullptr;
     uint8_t* d_mark = nullptr;
     uint64_t* d_cols = nullptr;
+    uint32_t* d_wins = nullptr;
     uint64_t stride = 0;
 };
 
@@ -202,8 +204,9 @@ void precompute_crc(clx_ctx* ctx, const uint8_t* bytes, const clx_frame_desc* de
 }
 
 void build_graph(clx_ctx* ctx, clx_batch* b);
-int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
-                 size_t out_elems, uint32_t batch_flags, uint32_t mode, size_t stride, clx_batch** out);
+int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
+                 const clx_frame_window* windows, size_t n_frames, size_t out_elems, uint32_t batch_flags, uint32_t mode,
+                 bool channels, uint32_t n_rows, size_t stride, clx_batch** out);
 
 // The interleaved modes hold a sample in 2 / 3 bytes only for frames of at most 16 / 24 bits per sample.
 bool frames_fit_mode(const clx_frame_desc* descs, size_t n_frames, uint32_t mode) {
@@ -423,7 +426,7 @@ int clx_decode_frames_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, cons
         CUD(cudaMemcpyAsync(sc.d_descs, ctx->h_descs + s.f0, nf * sizeof(clx_frame_desc), cudaMemcpyHostToDevice, st));
         // (never fused: no d_mark; the frame CRC-16 on the device, src/frame.rs:752-763)
         const clx::DecodeBuffers db{sc.d_bytes, nb_pad, sc.d_descs, (uint32_t)nf, sc.d_out, sc.d_results, sc.d_need_hi,
-                                    sc.d_params, mode, sc.d_conv, nullptr, nullptr, 0};
+                                    sc.d_params, mode, sc.d_conv, nullptr, nullptr, 0, nullptr};
         CUD(clx::launch_decode(db, plan, !(ctx->flags & CLX_OPT_NO_VERIFY_CRC), st, &ctx->launches));
         if (mode == CLX_OUT_PLANAR_I32)
             CUD(cudaMemcpyAsync(out + s.o0 * esize, sc.d_out + lead, no * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -472,39 +475,63 @@ int clx_batch_create_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const
     CU(ctx, cudaSetDevice(ctx->device));
     for (size_t i = 0; i < n_frames; i++)
         if (!valid_desc(descs[i], nbytes, out_elems)) return CLX_ERR_INVALID_ARGUMENT;
-    return create_batch(ctx, bytes, nbytes, descs, n_frames, out_elems, batch_flags, mode, 0, out);
+    return create_batch(ctx, bytes, nbytes, descs, nullptr, n_frames, out_elems, batch_flags, mode, false, 0, 0, out);
 }
 
 int clx_batch_create_channels(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
                               size_t n_frames, uint32_t n_channels, size_t channel_stride, uint32_t batch_flags,
                               uint32_t mode, clx_batch** out) {
-    if (!ctx || !out || (!bytes && nbytes) || (!descs && n_frames) ||
-        (mode != CLX_OUT_CHANNELS_I32 && mode != CLX_OUT_CHANNELS_F32))
-        return CLX_ERR_INVALID_ARGUMENT;
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
     *out = nullptr;
-    if (n_channels == 0 || n_channels > 8 || channel_stride == 0 || channel_stride > SIZE_MAX / 4 / n_channels)
-        return CLX_ERR_INVALID_ARGUMENT;
-    CU(ctx, cudaSetDevice(ctx->device));
-    for (size_t i = 0; i < n_frames; i++) {
-        const clx_frame_desc& d = descs[i];
-        clx_frame_desc at0 = d;  // the byte-range conditions, with the frame alone in its own output
-        at0.out_offset = 0;
-        if (!valid_desc(at0, nbytes, (size_t)d.n_channels * d.block_size) || d.n_channels > n_channels ||
-            d.out_offset > channel_stride || d.block_size > channel_stride - d.out_offset ||
-            (mode == CLX_OUT_CHANNELS_F32 && d.bits_per_sample > 24))
-            return CLX_ERR_INVALID_ARGUMENT;
-    }
-    return create_batch(ctx, bytes, nbytes, descs, n_frames, (size_t)n_channels * channel_stride, batch_flags, mode,
+    if (n_channels > 8) return CLX_ERR_INVALID_ARGUMENT;
+    return create_batch(ctx, bytes, nbytes, descs, nullptr, n_frames, 0, batch_flags, mode, true, n_channels,
                         channel_stride, out);
+}
+
+int clx_batch_create_windows(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
+                             const clx_frame_window* windows, size_t n_frames, uint32_t n_rows, size_t row_stride,
+                             uint32_t batch_flags, uint32_t mode, clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (!windows && n_frames) return CLX_ERR_INVALID_ARGUMENT;
+    return create_batch(ctx, bytes, nbytes, descs, windows, n_frames, 0, batch_flags, mode, true, n_rows, row_stride, out);
 }
 
 }  // extern "C"
 
 namespace {
-// The part of batch creation every mode shares, after the caller's arguments have been checked.  `stride` != 0: a
-// channels mode, out_elems = rows * stride.
-int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
-                 size_t out_elems, uint32_t batch_flags, uint32_t mode, size_t stride, clx_batch** out) {
+// Everything the channels modes require of a frame and its window (`w`: null for the full window at row 0), beyond
+// the byte-range conditions of valid_desc.
+bool valid_window(const clx_frame_desc& d, const clx_frame_window* w, size_t nbytes, uint32_t n_rows, size_t stride,
+                  uint32_t mode) {
+    const clx_frame_window full{0, 0, d.block_size, 0};
+    if (!w) w = &full;
+    clx_frame_desc at0 = d;  // the byte-range conditions, with the frame alone in its own output
+    at0.out_offset = 0;
+    return valid_desc(at0, nbytes, (size_t)d.n_channels * d.block_size) && w->reserved == 0 &&
+           w->row <= n_rows && d.n_channels <= n_rows - w->row && w->first < d.block_size && w->count != 0 &&
+           w->count <= (uint32_t)d.block_size - w->first && d.out_offset <= stride && w->count <= stride - d.out_offset &&
+           !(mode == CLX_OUT_CHANNELS_F32 && d.bits_per_sample > 24);
+}
+
+// The part of batch creation every mode shares.  !channels: a planar or interleaved mode, whose arguments the caller has
+// checked (n_rows = stride = 0).  `channels` (clx_batch_create_channels, _windows): a channels mode with `n_rows` rows,
+// out_elems = n_rows * stride, and each frame's window in `windows` (null: full windows at row 0); the arguments are
+// checked here.
+int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
+                 const clx_frame_window* windows, size_t n_frames, size_t out_elems, uint32_t batch_flags, uint32_t mode,
+                 bool channels, uint32_t n_rows, size_t stride, clx_batch** out) {
+    if (channels) {
+        if (!ctx || !out || (!bytes && nbytes) || (!descs && n_frames) ||
+            (mode != CLX_OUT_CHANNELS_I32 && mode != CLX_OUT_CHANNELS_F32))
+            return CLX_ERR_INVALID_ARGUMENT;
+        if (n_rows == 0 || stride == 0 || stride > SIZE_MAX / 4 / n_rows) return CLX_ERR_INVALID_ARGUMENT;
+        CU(ctx, cudaSetDevice(ctx->device));
+        for (size_t i = 0; i < n_frames; i++)
+            if (!valid_window(descs[i], windows ? &windows[i] : nullptr, nbytes, n_rows, stride, mode))
+                return CLX_ERR_INVALID_ARGUMENT;
+        out_elems = (size_t)n_rows * stride;
+    }
     const bool on_device = (batch_flags & CLX_BATCH_BYTES_ON_DEVICE) != 0;
     clx_batch* b = new clx_batch();
     b->nbytes = nbytes;
@@ -514,11 +541,13 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
     b->plan = make_plan(ctx, descs, n_frames);
     b->mode = mode;
     b->stride = stride;
-    // Device descriptors in the device order (shape_order); in a channels mode each frame's column moves to `cols` and
-    // out_offset becomes its place in the planar scratch, packed back to back, so that every planar kernel runs as is.
+    // Device descriptors in the device order (shape_order); in a channels mode each frame's window start moves to
+    // `cols` (row base * stride + column) and its window to `wins`, and out_offset becomes its place in the planar
+    // scratch, packed back to back, so that every planar kernel runs as is.
     const bool reordered = shape_order(descs, 0, n_frames, b->order);
     std::vector<clx_frame_desc> dev;
     std::vector<uint64_t> cols;
+    std::vector<uint32_t> wins;
     size_t planar_elems = out_elems;
     if (reordered || stride) {
         dev.resize(n_frames);
@@ -526,9 +555,13 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
     }
     if (stride) {
         cols.resize(n_frames);
+        wins.resize(n_frames);
         planar_elems = 0;
         for (size_t p = 0; p < n_frames; p++) {
-            cols[p] = dev[p].out_offset;
+            const size_t i = reordered ? b->order[p] : p;
+            const clx_frame_window w = windows ? windows[i] : clx_frame_window{0, 0, dev[p].block_size, 0};
+            cols[p] = (uint64_t)w.row * stride + dev[p].out_offset;
+            wins[p] = w.first | (w.count << 16);
             dev[p].out_offset = planar_elems;
             planar_elems += ((size_t)dev[p].n_channels * dev[p].block_size + 3) & ~(size_t)3;
         }
@@ -545,6 +578,8 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
     if (e == cudaSuccess && stride) e = cudaMemset(b->d_conv, 0, (out_elems + 8) * sizeof(int32_t));  // uncovered elements read 0
     if (e == cudaSuccess && stride) e = cudaMalloc((void**)&b->d_cols, std::max<size_t>(1, n_frames) * sizeof(uint64_t));
     if (e == cudaSuccess && stride) e = cudaMemcpy(b->d_cols, cols.data(), n_frames * sizeof(uint64_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && stride) e = cudaMalloc((void**)&b->d_wins, std::max<size_t>(1, n_frames) * sizeof(uint32_t));
+    if (e == cudaSuccess && stride) e = cudaMemcpy(b->d_wins, wins.data(), n_frames * sizeof(uint32_t), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(b->d_bytes, bytes, nbytes, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
     if (e == cudaSuccess)
         e = cudaMemcpy(b->d_descs, dev.empty() ? descs : dev.data(), n_frames * sizeof(clx_frame_desc), cudaMemcpyHostToDevice);
@@ -571,7 +606,7 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
 
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
     const clx::DecodeBuffers db{b->d_bytes, b->buf_bytes, b->d_descs, b->n_frames, b->d_out, b->d_results, b->d_need_hi,
-                                b->d_params, b->mode, b->d_conv, b->d_mark, b->d_cols, b->stride};
+                                b->d_params, b->mode, b->d_conv, b->d_mark, b->d_cols, b->stride, b->d_wins};
     return clx::launch_decode(db, b->plan, b->device_crc, st, launches);
 }
 
@@ -700,7 +735,7 @@ void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
     if (!b) return;
     cudaFree(b->d_bytes); cudaFree(b->d_descs); cudaFree(b->d_out); cudaFree(b->d_results); cudaFree(b->d_need_hi);
     cudaFree(b->d_params);
-    cudaFree(b->d_conv); cudaFree(b->d_mark); cudaFree(b->d_cols);
+    cudaFree(b->d_conv); cudaFree(b->d_mark); cudaFree(b->d_cols); cudaFree(b->d_wins);
     if (b->graph) cudaGraphExecDestroy(b->graph);
     if (b->ev_idle) cudaEventDestroy(b->ev_idle);
     if (b->ev_start) cudaEventDestroy(b->ev_start);

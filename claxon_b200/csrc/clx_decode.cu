@@ -692,8 +692,8 @@ cudaError_t launch_decode(const DecodeBuffers& b, const Plan& plan, bool crc, cu
                        (b.mode == CLX_OUT_INTERLEAVED_I32 || b.mode == CLX_OUT_INTERLEAVED_I16 || channels);
     // planar -> the batch's mode, for the frames in `sel` (all if null) unless *gate == 0
     auto convert = [&](const uint8_t* sel, const int* gate) {
-        return channels ? launch_channels(b.descs, b.n_frames, plan.max_frame_elems, b.out, b.conv, b.cols, b.stride, b.mode,
-                                          stream, launches, sel, gate)
+        return channels ? launch_channels(b.descs, b.n_frames, plan.max_frame_elems, b.out, b.conv, b.cols, b.stride, b.wins,
+                                          b.mode, stream, launches, sel, gate)
                         : launch_interleave(b.descs, b.n_frames, plan.max_frame_elems, b.out, b.conv, b.mode, stream,
                                             launches, sel, gate);
     };
@@ -705,7 +705,7 @@ cudaError_t launch_decode(const DecodeBuffers& b, const Plan& plan, bool crc, cu
     if (plan.path == Path::LanePerFrame)
         e = launch_seq(b.bytes, b.buf_bytes, b.descs, b.n_frames, fused ? static_cast<int32_t*>(b.conv) : b.out, b.results,
                        d_generic, d_need_wide, b.params, plan, fused ? b.mode : (uint32_t)CLX_OUT_PLANAR_I32, b.cols, b.stride,
-                       stream, launches);
+                       b.wins, stream, launches);
     else if (plan.path == Path::WarpPerFrame)
         e = launch_warp_per_frame(b.bytes, b.buf_bytes, b.descs, b.n_frames, b.out, b.results, d_generic, b.params, plan,
                                   stream, launches);

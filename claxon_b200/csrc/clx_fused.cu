@@ -323,12 +323,14 @@ using SubIO = DeviceIO<DEC_RQ, 3>;
 // little-endian integer of 4 / 2 bytes.  In the interleaved instances `out` is the FRAME's first element (the same
 // for all its rows), bit 0 of `meta` says that this address is 16-byte aligned, and bits 24-27 / 28-31 hold the
 // frame's channel count and the row's channel.
-// CLX_OUT_CHANNELS_I32 / _F32 write a channels-first buffer: `out` is the row's first element, `out + c * stride +
-// column`, and the flush takes the planar branches (rows are independent addresses).  In F32, bits 24-29 of `meta`
-// hold the frame header's bits_per_sample, whose power of two scales the row.
+// CLX_OUT_CHANNELS_I32 / _F32 write a channels-first buffer: a row stores only the steps of the frame's window
+// [lo, hi), `bs` holds lo << 16 | hi (a full window: the block size), and `out` is the address of step lo, the
+// window's first element (so that no address outside the buffer is ever formed): step g goes to out[g - lo].  The
+// flush takes the planar branches (rows are independent addresses).  In F32, bits 24-29 of `meta` hold the frame
+// header's bits_per_sample, whose power of two scales the row.
 struct __align__(16) SeqRow {
     int32_t* out;   // subframe's first output element (nullptr: idle row)
-    uint32_t bs;    // block size
+    uint32_t bs;    // block size (channels modes: the window, see above)
     uint32_t meta;  // bit 0: 16-byte stores allowed; bits 8-15: wasted bits; bits 16-19 (even rows): 8 left/side,
                     // 9 side/right, 10 mid/side, 0 independent
 };
@@ -384,6 +386,18 @@ __device__ __forceinline__ void seq_store_vec(int32_t* out, uint32_t bs, bool ve
         if (g + 3 < bs) out[g + 3] = v.w;
     }
 }
+// Channels-first: steps g .. g+3 of a row whose window is [lo, hi) (win = lo << 16 | hi), step s at out[s - lo].
+__device__ __forceinline__ void ch_store_vec(int32_t* out, uint32_t win, bool vec, uint32_t g, const int4& v) {
+    const uint32_t lo = win >> 16, hi = win & 0xffffu;
+    if (out == nullptr || g >= hi || g + 4 <= lo) return;
+    if (vec && g >= lo && g + 4 <= hi) *reinterpret_cast<int4*>(out + (g - lo)) = v;
+    else {
+        if (g >= lo) out[g - lo] = v.x;
+        if (g + 1 >= lo && g + 1 < hi) out[g + 1 - lo] = v.y;
+        if (g + 2 >= lo && g + 2 < hi) out[g + 2 - lo] = v.z;
+        if (g + 3 >= lo && g + 3 < hi) out[g + 3 - lo] = v.w;
+    }
+}
 __device__ __forceinline__ int4 shl4(const int4& v, uint32_t s) {
     return make_int4((int32_t)((uint32_t)v.x << s), (int32_t)((uint32_t)v.y << s), (int32_t)((uint32_t)v.z << s),
                      (int32_t)((uint32_t)v.w << s));
@@ -402,7 +416,8 @@ __device__ __forceinline__ void mid_side(int32_t& a, int32_t& b) {
 // bits (src/subframe.rs:216-225), decorrelation (src/frame.rs:319-389), planar i32.  Eight lanes take the eight
 // 16-byte vectors of a row pair (rows 2p, 2p+1), so each store instruction of the warp covers four whole
 // 128-byte lines — scattering the lanes over more rows costs the load/store unit a wavefront per line.
-// CHECKED = false is for tiles wholly inside every active row with 16-byte stores allowed everywhere.
+// CHECKED = false is for tiles wholly inside every active row with 16-byte stores allowed everywhere (channels-first:
+// rows whose windows are the whole block).
 // Channels-first: the planar stores, at the rows' own addresses; F32 converts after decorrelation.
 // Interleaved: a quarter holds whole frames (CH <= 8 channel slots, a frame's channels are CH
 // consecutive rows), and a lane writes what it holds: four interleaved pairs when its rows are a stereo frame's two
@@ -440,6 +455,9 @@ __device__ __forceinline__ void seq_flush_quarter(const int32_t* tile, const Seq
             il_store_row<OM>(i0, g, a);
             il_store_row<OM>(i1, g, b);
         }
+    } else if (is_channels(OM) && CHECKED) {
+        ch_store_vec(i0.out, i0.bs, (i0.meta & 1u) != 0, g, a);
+        ch_store_vec(i1.out, i1.bs, (i1.meta & 1u) != 0, g, b);
     } else if (CHECKED) {
         seq_store_vec(i0.out, i0.bs, (i0.meta & 1u) != 0, g, a);
         seq_store_vec(i1.out, i1.bs, (i1.meta & 1u) != 0, g, b);
@@ -509,6 +527,8 @@ __device__ __forceinline__ void flush_quarter_fast(uint32_t tile_s, uint32_t out
 //   tile_s: shared address of the warp's two tiles (8 KB, 8 KB-aligned: the other tile is `addr ^ 4096`).
 //   FMODE: 0 = general flush; 1 / 2 = flush_quarter_fast applies, without stereo decorrelation / mid-side.
 //   fs: channels-first F32 with FMODE != 0, the warp's one scale.
+//   all_vec: the unchecked general flush applies to the tiles of [head_end, bulk_end) (channels-first: only when every
+//   active row's window is its whole block).
 template <int TAPS, int U, typename ACC, int FMODE, int OM>
 __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint32_t order, uint32_t shift,
                                             const SeqParams* __restrict__ sp, bool active, int32_t* tile, uint32_t tile_s,
@@ -705,15 +725,16 @@ __device__ __forceinline__ void decode_rows(SubLane<SubIO>& L, uint32_t bs, uint
 //
 // OM: the output mode (see SeqRow).  The interleaved and channels instances write a frame's samples straight into the
 // batch's buffer `out`, after wasted bits and decorrelation as the planar flush applies them; the planar instance is
-// the one every other path shares.  `cols` / `stride` (channels instances only; the others ignore them): the frame's
-// column, per frame in the order of `descs`, and the row length of the channels buffer.
+// the one every other path shares.  `cols` / `stride` / `wins` (channels instances only; the others ignore them): per
+// frame in the order of `descs`, the element where the window starts on the frame's first row (row * stride + column);
+// the row length of the channels buffer; the window, first | count << 16 (the samples of the frame that are stored).
 template <int GROUP, bool WIDE, int OM = CLX_OUT_PLANAR_I32>
 __global__ void __launch_bounds__(DEC_WARPS * 32)
 decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, const clx_frame_desc* __restrict__ descs,
                         uint32_t n_frames, int32_t* __restrict__ out, clx_frame_result* __restrict__ results,
                         const SeqParams* __restrict__ params, uint32_t CH, uint32_t ch_log2, uint32_t n_pwarps,
                         int* __restrict__ need_generic, int* __restrict__ need_wide, const uint64_t* __restrict__ cols,
-                        uint64_t stride) {
+                        uint64_t stride, const uint32_t* __restrict__ wins) {
     __shared__ __align__(8192) int32_t s_tile[DEC_WARPS][2 * 32 * 32];  // two tiles: one fills while the other drains
     __shared__ SeqRow s_rows[DEC_WARPS][32];
     __shared__ __align__(16) int32_t* s_outp[DEC_WARPS][32];
@@ -734,6 +755,7 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
 
     bool active = false, narrow_ok = true, last = false;
     uint32_t bs = 0, order = 0, shift = 0, wasted = 0, ca = 0, absum = 0, bit0 = 0, byte_len = 0, il_meta = 0;
+    uint32_t win_lo = 0, win_hi = 0;  // channels-first: the row's window [lo, hi)
     const SeqParams* sp = params;
     int32_t* sub = nullptr;
     SubLane<SubIO> L;
@@ -753,7 +775,10 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
             absum = sp->absum;
             ca = d.channel_assignment >= 8 ? d.channel_assignment : 0u;
             if constexpr (OM == CLX_OUT_PLANAR_I32) sub = out + d.out_offset + (size_t)c * bs;
-            else if constexpr (is_channels(OM)) {  // the row's first element
+            else if constexpr (is_channels(OM)) {  // the row's first stored element
+                const uint32_t w = wins[f];
+                win_lo = w & 0xffffu;
+                win_hi = win_lo + (w >> 16);
                 sub = out + c * stride + cols[f];
                 if (OM == CLX_OUT_CHANNELS_F32) il_meta = (uint32_t)d.bits_per_sample << 24;
             } else {  // the frame's first interleaved element
@@ -774,13 +799,17 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
     const uint32_t max_order = __reduce_max_sync(0xffffffffu, active ? order : 0u);
     const int cls = max_order <= 8 ? 0 : max_order <= 12 ? 1 : 2;
     if ((cls == 2) != (GROUP == 1)) return;
-    const bool vec_own = (reinterpret_cast<uintptr_t>(sub) & 15) == 0;
-    const bool all_vec = __all_sync(0xffffffffu, !active || vec_own);
+    // (channels-first: judged at the address of a step that is a multiple of 4, sub + (g - lo))
+    const bool vec_own = ((reinterpret_cast<uintptr_t>(sub) - (is_channels(OM) ? 4u * win_lo : 0u)) & 15) == 0;
+    // (channels-first: a warp with a clipped row takes neither the straight-line flush nor the unchecked general flush,
+    // so that every step outside a window is checked)
+    const bool full_windows = !is_channels(OM) || __all_sync(0xffffffffu, !active || (win_lo == 0 && win_hi == bs));
+    const bool all_vec = full_windows && __all_sync(0xffffffffu, !active || vec_own);
     SeqRow* pr = s_rows[warp];
     {
         SeqRow row;
         row.out = sub;
-        row.bs = bs;
+        row.bs = is_channels(OM) ? (win_lo << 16) | win_hi : bs;
         row.meta = (vec_own ? 1u : 0u) | (wasted << 8) | ((c == 0 ? ca : 0u) << 16);
         if constexpr (OM != CLX_OUT_PLANAR_I32) row.meta |= il_meta;
         pr[lane] = row;
@@ -803,7 +832,7 @@ decode_subframes_kernel(const uint8_t* __restrict__ bytes, uint64_t buf_bytes, c
         one_scale = __all_sync(0xffffffffu, (il_meta >> 24) == bps0);
         fs = f32_scale(bps0);
     }
-    const bool fast_flush = (!is_interleaved(OM) || CH == 2) && one_scale &&
+    const bool fast_flush = (!is_interleaved(OM) || CH == 2) && one_scale && full_windows &&
                             __all_sync(0xffffffffu, active && vec_own && wasted == 0 && pair_ca == ca0);
     const int fmode = !fast_flush ? 0 : ca0 == 0 ? 1 : ca0 == 10 ? 2 : 0;
     int32_t smin = 0, smax = 0;
@@ -880,8 +909,8 @@ size_t seq_scratch_bytes(const Plan& plan, uint32_t n_frames) {
 
 cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
                        int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, int* d_need_wide, void* d_params,
-                       const Plan& plan, uint32_t mode, const uint64_t* d_cols, uint64_t stride, cudaStream_t stream,
-                       uint64_t* launches) {
+                       const Plan& plan, uint32_t mode, const uint64_t* d_cols, uint64_t stride, const uint32_t* d_wins,
+                       cudaStream_t stream, uint64_t* launches) {
 #ifdef CLX_EXPERIMENT
     const int which = g_exp_which;
 #else
@@ -909,7 +938,7 @@ cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_fra
     do {                                                                                                                  \
         decode_subframes_kernel<C, W, M><<<g2, b2, dyn, stream>>>(d_bytes, buf_bytes, d_descs, n_frames, d_out, d_results, \
                                                                   params, CH, ch_log2, n_pwarps, d_need_generic, d_need_wide, \
-                                                                  d_cols, stride);                                        \
+                                                                  d_cols, stride, d_wins);                                \
         (*launches)++;                                                                                                    \
     } while (0)
 #define CLX_DEC4(M)                                                      \

@@ -39,8 +39,10 @@ size_t seq_scratch_bytes(const Plan& plan, uint32_t n_frames);
 // output in mode CLX_OUT_PLANAR_I32, else the generic kernel's scratch); `conv`: the output of an interleaved or
 // channels mode.  `mark` (one byte per frame, optional): given, a LanePerFrame decode to interleaved I32 / I16 or to a
 // channels mode writes `conv` itself; `mark` then records which frames the generic kernel takes over, and only those
-// are converted after it.  Channels modes only: `cols`, the column of each frame in the order of `descs` (whose
-// out_offset is then the frame's place in the planar scratch `out`), and `stride`, the row length of `conv`.
+// are converted after it.  Channels modes only: `cols`, per frame in the order of `descs` (whose out_offset is then the
+// frame's place in the planar scratch `out`), the element of `conv` where the frame's window starts on its first row
+// (row base * stride + column); `stride`, the row length of `conv`; `wins`, the frame's window, first | count << 16:
+// samples [first, first + count) of each channel are stored, no other element is written.
 struct DecodeBuffers {
     const uint8_t* bytes;
     uint64_t buf_bytes;
@@ -55,6 +57,7 @@ struct DecodeBuffers {
     uint8_t* mark;
     const uint64_t* cols;
     uint64_t stride;
+    const uint32_t* wins;
 };
 // The whole launch sequence of one decode on `stream`: the plan's kernels, the device CRC-16 when `crc`, the
 // conversion to an interleaved mode.  Every kernel launched adds one to *launches.
@@ -65,11 +68,11 @@ cudaError_t launch_warp_per_frame(const uint8_t* d_bytes, uint64_t buf_bytes, co
                                   int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, void* d_params,
                                   const Plan& plan, cudaStream_t stream, uint64_t* launches);
 // `mode`: the output mode the decode pass writes (planar, or interleaved I32 / I16 or channels I32 / F32 into `d_out`;
-// `d_cols` / `stride` as in DecodeBuffers).
+// `d_cols` / `stride` / `d_wins` as in DecodeBuffers).
 cudaError_t launch_seq(const uint8_t* d_bytes, uint64_t buf_bytes, const clx_frame_desc* d_descs, uint32_t n_frames,
                        int32_t* d_out, clx_frame_result* d_results, int* d_need_generic, int* d_need_wide, void* d_params,
-                       const Plan& plan, uint32_t mode, const uint64_t* d_cols, uint64_t stride, cudaStream_t stream,
-                       uint64_t* launches);
+                       const Plan& plan, uint32_t mode, const uint64_t* d_cols, uint64_t stride, const uint32_t* d_wins,
+                       cudaStream_t stream, uint64_t* launches);
 // clx_crc.cu: frame CRC-16 of every frame that decoded (over the length the decode found), on the device
 cudaError_t crc16_init();  // once per context, on its device
 cudaError_t launch_crc16(const uint8_t* d_bytes, const clx_frame_desc* d_descs, uint32_t n_frames, clx_frame_result* d_results,
@@ -80,10 +83,11 @@ uint32_t output_elem_size(uint32_t mode);
 cudaError_t launch_interleave(const clx_frame_desc* d_descs, uint32_t n_frames, uint32_t max_frame_elems, const int32_t* d_planar,
                               void* d_dst, uint32_t mode, cudaStream_t stream, uint64_t* launches, const uint8_t* sel = nullptr,
                               const int* gate = nullptr);
-// planar i32 -> channels-first i32 / f32 (CLX_OUT_CHANNELS_*): row c of frame f at d_dst + c * stride + d_cols[f].
-// `sel` / `gate` as for launch_interleave.
+// planar i32 -> channels-first i32 / f32 (CLX_OUT_CHANNELS_*): samples [first, first + count) of channel c of frame f
+// (d_wins[f] = first | count << 16) at d_dst + c * stride + d_cols[f].  `sel` / `gate` as for launch_interleave.
 cudaError_t launch_channels(const clx_frame_desc* d_descs, uint32_t n_frames, uint32_t max_frame_elems, const int32_t* d_planar,
-                            void* d_dst, const uint64_t* d_cols, uint64_t stride, uint32_t mode, cudaStream_t stream,
+                            void* d_dst, const uint64_t* d_cols, uint64_t stride, const uint32_t* d_wins, uint32_t mode,
+                            cudaStream_t stream,
                             uint64_t* launches, const uint8_t* sel = nullptr, const int* gate = nullptr);
 // mark[f] = (results[f].status == status) for every frame, unless *gate == 0 (then nothing is written).
 cudaError_t launch_mark_status(const clx_frame_result* d_results, uint32_t n_frames, int32_t status, uint8_t* d_mark,

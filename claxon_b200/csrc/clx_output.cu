@@ -50,27 +50,30 @@ interleave_kernel(const clx_frame_desc* __restrict__ descs, uint32_t n_frames, c
     }
 }
 
-// Channels-first: one CTA per (tile, frame) as above.  Element i of a frame's planar block is sample t = i % block_size
-// of channel c = i / block_size, which goes to row c at column cols[f] + t: reads and writes are coalesced along each
-// row.  F32: (float)s * 2^-(bits_per_sample - 1), rounded to nearest even, as the decode pass's channels flush.
+// Channels-first: one CTA per (tile, frame) as above, over the frame's window only: samples [first, first + count) of
+// each channel (wins[f] = first | count << 16).  Element i of the window is sample first + t of channel c (i = c * count
+// + t), which goes to row c at element cols[f] + t of the buffer: reads and writes are coalesced along each row, and
+// nothing outside the window is written.  F32: (float)s * 2^-(bits_per_sample - 1), rounded to nearest even, as the
+// decode pass's channels flush.
 template <bool F32>
 __global__ void __launch_bounds__(256)
 channels_kernel(const clx_frame_desc* __restrict__ descs, uint32_t n_frames, const int32_t* __restrict__ planar,
-                int32_t* __restrict__ dst, const uint64_t* __restrict__ cols, uint64_t stride, const uint8_t* __restrict__ sel,
-                const int* __restrict__ gate) {
+                int32_t* __restrict__ dst, const uint64_t* __restrict__ cols, uint64_t stride,
+                const uint32_t* __restrict__ wins, const uint8_t* __restrict__ sel, const int* __restrict__ gate) {
     if (gate != nullptr && *gate == 0) return;
     const uint32_t f = blockIdx.y;
     if (f >= n_frames || (sel != nullptr && sel[f] == 0)) return;
     const clx_frame_desc d = descs[f];
-    const uint32_t bs = d.block_size, total = (uint32_t)d.n_channels * bs;
+    const uint32_t bs = d.block_size, first = wins[f] & 0xffffu, count = wins[f] >> 16;
+    const uint32_t total = (uint32_t)d.n_channels * count;
     const uint32_t base = blockIdx.x * IL_TILE;
     if (base >= total) return;
-    const int32_t* src = planar + d.out_offset;
+    const int32_t* src = planar + d.out_offset + first;
     int32_t* out = dst + cols[f];
     const float scale = __int_as_float((int)(128u - d.bits_per_sample) << 23);  // 2^-(bps-1)
     for (uint32_t i = base + threadIdx.x; i < min(base + IL_TILE, total); i += 256) {
-        const uint32_t c = i / bs, t = i - c * bs;
-        const int32_t v = src[i];
+        const uint32_t c = i / count, t = i - c * count;
+        const int32_t v = src[c * bs + t];
         out[c * stride + t] = F32 ? __float_as_int(__fmul_rn(__int2float_rn(v), scale)) : v;
     }
 }
@@ -100,8 +103,8 @@ cudaError_t launch_interleave(const clx_frame_desc* d_descs, uint32_t n_frames, 
 }
 
 cudaError_t launch_channels(const clx_frame_desc* d_descs, uint32_t n_frames, uint32_t max_frame_elems, const int32_t* d_planar,
-                            void* d_dst, const uint64_t* d_cols, uint64_t stride, uint32_t mode, cudaStream_t stream,
-                            uint64_t* launches, const uint8_t* sel, const int* gate) {
+                            void* d_dst, const uint64_t* d_cols, uint64_t stride, const uint32_t* d_wins, uint32_t mode,
+                            cudaStream_t stream, uint64_t* launches, const uint8_t* sel, const int* gate) {
     if (n_frames == 0) return cudaSuccess;
     const uint32_t tiles = (max_frame_elems + IL_TILE - 1) / IL_TILE;
     for (uint32_t f0 = 0; f0 < n_frames; f0 += 65535) {  // gridDim.y limit
@@ -109,9 +112,11 @@ cudaError_t launch_channels(const clx_frame_desc* d_descs, uint32_t n_frames, ui
         dim3 grid(tiles, nf);
         const uint8_t* s = sel ? sel + f0 : nullptr;
         if (mode == CLX_OUT_CHANNELS_F32)
-            channels_kernel<true><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (int32_t*)d_dst, d_cols + f0, stride, s, gate);
+            channels_kernel<true><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (int32_t*)d_dst, d_cols + f0, stride,
+                                                            d_wins + f0, s, gate);
         else
-            channels_kernel<false><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (int32_t*)d_dst, d_cols + f0, stride, s, gate);
+            channels_kernel<false><<<grid, 256, 0, stream>>>(d_descs + f0, nf, d_planar, (int32_t*)d_dst, d_cols + f0, stride,
+                                                            d_wins + f0, s, gate);
     }
     (*launches)++;  // one pass, however many grids its frames need
     return cudaGetLastError();

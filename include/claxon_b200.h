@@ -243,6 +243,30 @@ int clx_batch_create_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const
 int clx_batch_create_channels(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
                               size_t n_frames, uint32_t n_channels, size_t channel_stride, uint32_t batch_flags,
                               uint32_t mode, clx_batch** out);
+/* Channels-first output of sample ranges: each frame stores only a window of its samples, on rows of its own.  This is
+ * what a batch of excerpts ("4 s from a random offset of each of B files") needs: the frames that overlap an excerpt
+ * are decoded, the first and last of them clipped to it, each excerpt on rows of its own ([B * C, stride] rows).
+ * Channel c of frame i goes to row windows[i].row + c; its samples [first, first + count) go to columns
+ * [out_offset, out_offset + count) of that row (descs[i].out_offset is the column where sample `first` lands).  No
+ * element outside a frame's window is ever written; everything else is as for clx_batch_create_channels (wasted bits
+ * and decorrelation applied, the F32 rule, the buffer zeroed once at creation, a failed frame's window overwritten
+ * with what the planar layout holds for those samples, converted; clx_batch_read_to, clx_batch_device_out and
+ * CLX_BATCH_BYTES_ON_DEVICE as there).  The window {0, 0, block_size} on every frame gives, bit for bit, what
+ * clx_batch_create_channels gives.  n_rows has no cap of 8.  Overlapping windows are the caller's business; two
+ * descriptors may name the same frame bytes, each is decoded for its own window.
+ * CLX_ERR_INVALID_ARGUMENT for: windows NULL with frames, n_rows or row_stride 0, n_rows * row_stride * 4 overflowing,
+ * row + n_channels > n_rows, first >= block_size, count 0 or first + count > block_size, out_offset + count >
+ * row_stride, reserved != 0, in F32 a frame with bits_per_sample above 24, a mode other than CLX_OUT_CHANNELS_I32 /
+ * _F32, and every byte-range condition of the other create calls. */
+typedef struct clx_frame_window {
+    uint32_t row;      /* channel c of the frame goes to row `row + c` */
+    uint32_t first;    /* first sample of the frame that is stored, < block_size */
+    uint32_t count;    /* samples stored: 1 .. block_size - first */
+    uint32_t reserved; /* 0 */
+} clx_frame_window;
+int clx_batch_create_windows(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
+                             const clx_frame_window* windows, size_t n_frames, uint32_t n_rows, size_t row_stride,
+                             uint32_t batch_flags, uint32_t mode, clx_batch** out);
 int clx_batch_decode(clx_ctx* ctx, clx_batch* b, uint32_t stream_index); /* async on an internal stream */
 int clx_batch_sync(clx_ctx* ctx, clx_batch* b);
 /* Planar batches only (CLX_ERR_INVALID_ARGUMENT for any other mode). */

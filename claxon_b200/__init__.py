@@ -27,7 +27,8 @@ from ._lib import (FrameDesc, FrameResult, FrameWindow, OPT_NO_VERIFY_CRC, OPT_G
 
 __all__ = ["Error", "Block", "FrameReader", "FlacReader", "FlacReaderOptions", "StreamInfo", "Context", "DeviceBatch",
            "parse_frame_header", "demux_frames", "open_stream", "ogg_frames", "mp4_frames", "status_str", "DESC_DTYPE", "RESULT_DTYPE", "load", "plan_columns",
-           "WINDOW_DTYPE", "index", "FlacIndex", "IndexedFile", "load_crops", "plan_range", "frame_starts"]
+           "WINDOW_DTYPE", "index", "FlacIndex", "IndexedFile", "load_crops", "plan_range", "frame_starts", "Corpus",
+           "CropBatch"]
 
 # numpy views of the C structs (same layout; asserted below)
 DESC_DTYPE = np.dtype([
@@ -922,3 +923,178 @@ def load_crops(index: FlacIndex, files, offsets, num_frames: int, dtype=None, ct
         _decode_excerpts(index, excerpts, B * C_, num_frames, out.view(B * C_, num_frames), ctx,
                          lambda k: f"file {files[k]}, crop {k}")
     return out, lengths
+
+
+# ---------------------------------------------------------------------------
+# device-resident corpora: crops planned on the device
+# ---------------------------------------------------------------------------
+
+class _DeviceView:
+    """__cuda_array_interface__ of device memory owned by `owner`, which it keeps alive while a tensor views it."""
+
+    def __init__(self, owner, ptr: int, shape: tuple, typestr: str):
+        self.owner = owner
+        self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (int(ptr), False), "strides": None,
+                                         "version": 2}
+
+
+class Corpus:
+    """The compressed frames of a FlacIndex's files, uploaded to the GPU once with their frame index
+    (clx_corpus_create), for CropBatch: crops whose frames, windows and columns are planned on the device.  Each file's
+    bytes from its first frame to its end are uploaded; the trailing-bytes verdict of a file whose last frame's end is
+    unconfirmed is taken once here.  `index` is kept for error messages."""
+
+    def __init__(self, index: FlacIndex, ctx: Context | None = None):
+        self.index = index
+        self.ctx = ctx or default_context()
+        chunks, parts, file_frames, at = [], [], [0], 0
+        for f in index.files:
+            if f.descs.size:
+                b0 = int(f.descs["byte_offset"][0])
+                chunks.append(np.asarray(f.data[b0:]))
+                d = f.descs.copy()
+                d["byte_offset"] = d["byte_offset"] - np.uint64(b0) + np.uint64(at)
+                d["out_offset"] = 0
+                parts.append(d)
+                at += f.data.size - b0
+            file_frames.append(file_frames[-1] + f.descs.size)
+        data = np.concatenate(chunks) if chunks else np.zeros(0, np.uint8)
+        self.descs = np.concatenate(parts) if parts else np.zeros(0, dtype=DESC_DTYPE)
+        self.file_frames = np.array(file_frames, dtype=np.uint32)
+        self.nbytes = int(data.size)
+        self.channels = max([int(self.descs["n_channels"].max())] if self.descs.size else [1])
+        h = C.c_void_p()
+        _check(self.ctx._L.clx_corpus_create(self.ctx._h, data.ctypes.data, data.size, self.descs.ctypes.data,
+                                             self.descs.size, self.file_frames.ctypes.data, len(index), C.byref(h)), self.ctx)
+        self._h = h
+
+    def frames_bound(self, num_frames: int) -> int:
+        """clx_crop_frames_bound: the most frames num_frames consecutive samples of one file can overlap."""
+        return int(self.ctx._L.clx_crop_frames_bound(self.descs.ctypes.data, self.descs.size, self.file_frames.ctypes.data,
+                                                     len(self.index), int(num_frames)))
+
+    def crops(self, batch: int, num_frames: int, dtype=None) -> "CropBatch":
+        """A CropBatch of `batch` crops of `num_frames` samples; its CUDA graph is instantiated here."""
+        return CropBatch(self, batch, num_frames, dtype)
+
+    def close(self):
+        """Frees the device copy; raises Error while a CropBatch of the corpus is alive."""
+        if getattr(self, "_h", None) and getattr(self.ctx, "_h", None):
+            _check(self.ctx._L.clx_corpus_destroy(self.ctx._h, self._h), self.ctx)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class _CropHandle:
+    """Owns a crop batch's clx_batch; the tensors that view its buffers keep it (and its corpus) alive."""
+
+    def __init__(self, corpus: Corpus, h):
+        self.corpus, self.ctx, self.h = corpus, corpus.ctx, h
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.ctx, "_h", None):
+            self.ctx._L.clx_batch_destroy(self.ctx._h, self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class CropBatch:
+    """`batch` excerpts of `num_frames` samples of a Corpus's files per call, as one [B, C, L] CUDA tensor
+    (clx_batch_create_crops): the crops' frames, windows and columns are planned on the device inside the batch's CUDA
+    graph, so a call is two small device-to-device copies and one graph launch, and the offsets may be CUDA tensors
+    (drawn with torch.randint on the device, no sync).  C is the corpus's largest channel count.
+
+    Crop b is samples [offsets[b], offsets[b] + L) of file files[b], cut at the file's end: columns past it and rows the
+    file does not have read 0, as in load_crops(), whose results a call reproduces bit for bit.  `out` and `lengths`
+    (and `status`, an int32 CUDA tensor of per-crop statuses) are views of the batch's own buffers, overwritten by the
+    next call; the next call waits for what torch's current stream has enqueued before it, so reading them on that stream
+    is safe, clone() them to keep them.  Unlike load_crops(), a float32 batch is refused when any frame of the corpus
+    has more than 24 bits (load_crops() refuses only the frames a call selects)."""
+
+    def __init__(self, corpus: Corpus, batch: int, num_frames: int, dtype=None):
+        import torch
+        dtype = _torch_dtype(dtype)
+        self.corpus, self.ctx = corpus, corpus.ctx
+        self.batch, self.num_frames, self.dtype = int(batch), int(num_frames), dtype
+        if self.batch < 1 or self.num_frames < 1:
+            raise ValueError("batch and num_frames must be >= 1")
+        mode = OUT_CHANNELS_F32 if dtype == torch.float32 else OUT_CHANNELS_I32
+        L = self.ctx._L
+        h = C.c_void_p()
+        _check(L.clx_batch_create_crops(self.ctx._h, corpus._h, self.batch, self.num_frames, mode, C.byref(h)), self.ctx)
+        self._handle = _CropHandle(corpus, h)
+        self.channels = corpus.channels
+        B, hd = self.batch, self._handle
+
+        def view(ptr, shape, typestr):
+            return torch.as_tensor(_DeviceView(hd, ptr, shape, typestr), device="cuda")
+        self.out = view(L.clx_batch_device_out(h), (B, self.channels, self.num_frames),
+                        "<f4" if mode == OUT_CHANNELS_F32 else "<i4")
+        self.lengths = view(L.clx_batch_crop_lengths(h), (B,), "<i8")
+        self.status = view(L.clx_batch_crop_status(h), (B,), "<i4")
+        self._requests = view(L.clx_batch_crop_requests(h), (B, 2), "<i8")  # {u32 file, u32 reserved} as one i64, offset
+        self._error = view(L.clx_batch_crop_error(h), (1,), "<i8")
+        self._stream = torch.cuda.ExternalStream(L.clx_ctx_stream(self.ctx._h, 0))
+
+    def _column(self, x, what: str):
+        import torch
+        if isinstance(x, torch.Tensor):
+            if x.dtype.is_floating_point or x.dtype.is_complex or x.dtype == torch.bool:
+                raise TypeError(f"{what} must hold integers")
+            t = x.reshape(-1)
+        else:
+            t = torch.from_numpy(np.asarray(x, dtype=np.int64).reshape(-1))
+        if t.numel() != self.batch:
+            raise ValueError(f"{what}: {t.numel()} values for a batch of {self.batch}")
+        if not t.is_cuda:
+            t = t.to(torch.int64).pin_memory().to("cuda", non_blocking=True)
+        return t
+
+    def __call__(self, files, offsets, check: bool = True):
+        """Decodes crop b = samples [offsets[b], offsets[b] + L) of file files[b] for every b.  Returns (out [B, C, L],
+        lengths [B] int64), both on the GPU.  The requests are copied on torch's current stream, the batch's stream
+        waits for it, and torch's stream waits for the decode: nothing syncs with the host unless `check`.  check=True
+        syncs once and raises what load_crops() would: ValueError for the first crop whose file index or offset is out
+        of range, else Error(status, "file i, crop b") for the first crop with a failed frame, else for the first crop
+        that contains an unconfirmed last frame followed by something other than the end of the stream.  With
+        check=False nothing is raised; `status` holds each crop's outcome (CLX_ERR_INVALID_ARGUMENT, 90, for a request
+        out of range, whose rows are zero and length 0) and a failed crop's rows are unspecified."""
+        import torch
+        files, offsets = self._column(files, "files"), self._column(offsets, "offsets")
+        self._requests[:, 0].copy_(files)
+        self._requests[:, 1].copy_(offsets)
+        self._stream.wait_stream(torch.cuda.current_stream())
+        _check(self.ctx._L.clx_batch_decode(self.ctx._h, self._handle.h, 0), self.ctx)
+        torch.cuda.current_stream().wait_stream(self._stream)
+        if check:
+            self._raise()
+        return self.out, self.lengths
+
+    def _raise(self):
+        err = int(self._error.item()) & ((1 << 64) - 1)  # the one sync
+        if err == (1 << 64) - 1:
+            return
+        kind, b, st = err >> 62, (err >> 32) & ((1 << 30) - 1), err & 0xffffffff
+        st = st - (1 << 32) if st >= 1 << 31 else st
+        fi, o = (int(v) for v in self._requests[b].tolist())
+        if kind == 0:
+            if not 0 <= fi < len(self.corpus.index):
+                raise ValueError(f"crop {b}: file index {fi} out of range")
+            raise ValueError(f"crop {b}: offset {o} outside file {fi} ({self.corpus.index[fi].length} samples)")
+        raise Error(st, f"file {fi}, crop {b}")
+
+    def kernel_ms(self) -> float:
+        """Device time of the last call's graph (CUDA events), planner and status pass included."""
+        ms = C.c_float(0)
+        _check(self.ctx._L.clx_batch_last_kernel_ms(self.ctx._h, self._handle.h, C.byref(ms)), self.ctx)
+        return float(ms.value)

@@ -89,6 +89,15 @@ SYMBOLS = {
                                             C.POINTER(_vp)]),
     "clx_batch_create_windows": (C.c_int, [_vp, _u8p, _sz, _vp, _vp, _sz, C.c_uint32, _sz, C.c_uint32, C.c_uint32,
                                            C.POINTER(_vp)]),
+    "clx_corpus_create": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _vp, _sz, C.POINTER(_vp)]),
+    "clx_corpus_destroy": (C.c_int, [_vp, _vp]),
+    "clx_crop_frames_bound": (_sz, [_vp, _sz, _vp, _sz, _sz]),
+    "clx_batch_create_crops": (C.c_int, [_vp, _vp, _sz, _sz, C.c_uint32, C.POINTER(_vp)]),
+    "clx_batch_crop_requests": (_vp, [_vp]),
+    "clx_batch_crop_status": (_vp, [_vp]),
+    "clx_batch_crop_lengths": (_vp, [_vp]),
+    "clx_batch_crop_error": (_vp, [_vp]),
+    "clx_crop_filler_frame": (_sz, [_vp, _sz]),
     "clx_batch_decode": (C.c_int, [_vp, _vp, C.c_uint32]),
     "clx_batch_sync": (C.c_int, [_vp, _vp]),
     "clx_batch_read": (C.c_int, [_vp, _vp, _vp, _sz, _vp]),

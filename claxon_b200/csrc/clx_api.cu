@@ -150,6 +150,28 @@ struct clx_batch {
     uint64_t* d_cols = nullptr;
     uint32_t* d_wins = nullptr;
     uint64_t stride = 0;
+    // Crop batches (clx_batch_create_crops): d_bytes is the corpus's, not the batch's; the planner writes d_descs,
+    // d_cols and d_wins in every decode (clx_crops.cu).
+    clx_corpus* corpus = nullptr;
+    clx::CropBuffers crop{};
+};
+
+struct clx_corpus {
+    uint8_t* d_bytes = nullptr; size_t nbytes = 0, buf_bytes = 0;
+    clx_frame_desc* d_descs = nullptr;  // n_frames + 1: the filler frame last
+    int64_t* d_starts = nullptr;
+    uint32_t* d_file_frames = nullptr;
+    int64_t* d_file_len = nullptr;
+    uint32_t* d_file_ch = nullptr;
+    int32_t* d_file_tail = nullptr;
+    uint32_t n_frames = 0, n_files = 0;
+    std::vector<clx_frame_desc> descs;  // host copy, the filler frame last
+    std::vector<uint32_t> file_frames;
+    uint32_t channels = 1, max_bps = 0;
+    int live = 0;  // crop batches of this corpus
+    clx::CropCorpus view() const {
+        return {d_descs, d_starts, d_file_frames, d_file_len, d_file_ch, d_file_tail, n_files, n_frames};
+    }
 };
 
 namespace {
@@ -607,6 +629,7 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
     const clx::DecodeBuffers db{b->d_bytes, b->buf_bytes, b->d_descs, b->n_frames, b->d_out, b->d_results, b->d_need_hi,
                                 b->d_params, b->mode, b->d_conv, b->d_mark, b->d_cols, b->stride, b->d_wins};
+    if (b->corpus) return clx::launch_crops(b->corpus->view(), b->crop, db, b->plan, b->device_crc, st, launches);
     return clx::launch_decode(db, b->plan, b->device_crc, st, launches);
 }
 
@@ -733,7 +756,14 @@ int clx_batch_read_to(clx_ctx* ctx, clx_batch* b, void* out, size_t out_elems, c
 void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
     (void)ctx;
     if (!b) return;
-    cudaFree(b->d_bytes); cudaFree(b->d_descs); cudaFree(b->d_out); cudaFree(b->d_results); cudaFree(b->d_need_hi);
+    if (b->corpus) {  // the bytes are the corpus's
+        b->corpus->live--;
+        cudaFree((void*)b->crop.requests); cudaFree(b->crop.status); cudaFree(b->crop.lengths); cudaFree(b->crop.error);
+        cudaFree(b->crop.plan); cudaFree(b->crop.scan);
+    } else {
+        cudaFree(b->d_bytes);
+    }
+    cudaFree(b->d_descs); cudaFree(b->d_out); cudaFree(b->d_results); cudaFree(b->d_need_hi);
     cudaFree(b->d_params);
     cudaFree(b->d_conv); cudaFree(b->d_mark); cudaFree(b->d_cols); cudaFree(b->d_wins);
     if (b->graph) cudaGraphExecDestroy(b->graph);
@@ -795,6 +825,196 @@ void* clx_host_alloc(size_t bytes) {
     return p;
 }
 void clx_host_free(void* p) { if (p) cudaFreeHost(p); }
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------
+// device-resident corpora and crop batches (the kernels: clx_crops.cu)
+// ---------------------------------------------------------------------------------
+namespace {
+void free_corpus(clx_corpus* c) {
+    cudaFree(c->d_bytes); cudaFree(c->d_descs); cudaFree(c->d_starts); cudaFree(c->d_file_frames);
+    cudaFree(c->d_file_len); cudaFree(c->d_file_ch); cudaFree(c->d_file_tail);
+    delete c;
+}
+
+// The trailing-bytes verdict of a file whose last frame `d` has an unconfirmed end (load()'s check after the last
+// frame): decode the frame; if it decodes and ends before byte_len, the frame header status at its end, unless CLX_EOF.
+int tail_verdict(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, clx_frame_desc d, int32_t* verdict) {
+    *verdict = CLX_OK;
+    d.out_offset = 0;
+    std::vector<int32_t> pcm((size_t)d.n_channels * d.block_size);
+    clx_frame_result res{};
+    const int rc = clx_decode_frames(ctx, bytes, nbytes, &d, 1, pcm.data(), pcm.size(), &res);
+    if (rc) return rc;
+    if (res.status == CLX_OK && res.consumed < d.byte_len) {
+        clx_frame_desc next;
+        const uint64_t at = d.byte_offset + res.consumed;
+        const int st = clx_parse_frame_header(bytes + at, d.byte_offset + d.byte_len - at, &next, 0);
+        if (st != CLX_EOF && st != CLX_OK) *verdict = st;
+    }
+    return CLX_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int clx_corpus_create(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
+                      const uint32_t* file_frames, size_t n_files, clx_corpus** out) {
+    if (!ctx || !out || (!bytes && nbytes) || (!descs && n_frames) || !file_frames) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (n_frames >= UINT32_MAX || n_files >= UINT32_MAX || file_frames[n_files] != n_frames) return CLX_ERR_INVALID_ARGUMENT;
+    for (size_t i = 0; i < n_files; i++)
+        if (file_frames[i + 1] < file_frames[i]) return CLX_ERR_INVALID_ARGUMENT;
+    for (size_t i = 0; i < n_frames; i++) {
+        clx_frame_desc at0 = descs[i];  // the byte-range conditions, with the frame alone in its own output
+        at0.out_offset = 0;
+        if (!valid_desc(at0, nbytes, (size_t)descs[i].n_channels * descs[i].block_size)) return CLX_ERR_INVALID_ARGUMENT;
+    }
+    CU(ctx, cudaSetDevice(ctx->device));
+    clx_corpus* c = new clx_corpus();
+    c->n_frames = (uint32_t)n_frames;
+    c->n_files = (uint32_t)n_files;
+    c->nbytes = nbytes;
+    c->file_frames.assign(file_frames, file_frames + n_files + 1);
+    c->descs.assign(descs, descs + n_frames);
+    std::vector<int64_t> starts(n_frames), file_len(n_files);
+    std::vector<uint32_t> file_ch(n_files, 0);
+    std::vector<int32_t> tail(n_files, CLX_OK);
+    for (size_t i = 0; i < n_files; i++) {
+        int64_t at = 0;
+        for (size_t f = file_frames[i]; f < file_frames[i + 1]; f++) {
+            if (descs[f].n_channels != descs[file_frames[i]].n_channels) {
+                delete c;
+                return CLX_ERR_INVALID_ARGUMENT;
+            }
+            starts[f] = at;
+            at += descs[f].block_size;
+            c->channels = std::max<uint32_t>(c->channels, descs[f].n_channels);
+            c->max_bps = std::max<uint32_t>(c->max_bps, descs[f].bits_per_sample);
+        }
+        file_len[i] = at;
+        if (file_frames[i + 1] > file_frames[i]) {
+            const clx_frame_desc& last = descs[file_frames[i + 1] - 1];
+            file_ch[i] = last.n_channels;
+            if (!(last.flags & CLX_FRAME_CRC16_VERIFIED)) {
+                const int rc = tail_verdict(ctx, bytes, nbytes, last, &tail[i]);
+                if (rc) { delete c; return rc; }
+            }
+        }
+    }
+    uint8_t filler[16];
+    const size_t filler_len = clx::filler_frame(filler, sizeof filler);
+    clx_frame_desc fd;
+    const int fst = clx_parse_frame_header(filler, filler_len, &fd, 0);
+    if (fst != CLX_OK) { delete c; return fst; }
+    fd.byte_offset = nbytes;
+    fd.byte_len = (uint32_t)filler_len;
+    fd.flags |= CLX_FRAME_CRC16_VERIFIED;
+    fd.out_offset = 0;
+    c->descs.push_back(fd);
+    c->buf_bytes = ((nbytes + filler_len + 63) & ~(size_t)63) + 128;  // whole 64-byte TMA chunks + look-ahead
+    cudaError_t e = cudaMalloc((void**)&c->d_bytes, c->buf_bytes);
+    if (e == cudaSuccess) e = cudaMemset(c->d_bytes, 0, c->buf_bytes);
+    if (e == cudaSuccess && nbytes) e = cudaMemcpy(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(c->d_bytes + nbytes, filler, filler_len, cudaMemcpyHostToDevice);
+    auto put = [&](auto*& dst, const auto& v) {
+        if (e == cudaSuccess) e = cudaMalloc((void**)&dst, std::max<size_t>(1, v.size()) * sizeof(v[0]));
+        if (e == cudaSuccess && !v.empty()) e = cudaMemcpy(dst, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice);
+    };
+    put(c->d_descs, c->descs);
+    put(c->d_starts, starts);
+    put(c->d_file_frames, c->file_frames);
+    put(c->d_file_len, file_len);
+    put(c->d_file_ch, file_ch);
+    put(c->d_file_tail, tail);
+    if (e != cudaSuccess) {
+        free_corpus(c);
+        return cuda_fail(ctx, e, "clx_corpus_create");
+    }
+    *out = c;
+    return CLX_OK;
+}
+
+int clx_corpus_destroy(clx_ctx* ctx, clx_corpus* corpus) {
+    (void)ctx;
+    if (!corpus) return CLX_OK;
+    if (corpus->live > 0) return CLX_ERR_INVALID_ARGUMENT;
+    free_corpus(corpus);
+    return CLX_OK;
+}
+
+int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, size_t num_frames, uint32_t mode,
+                           clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (!ctx || !corpus || n_crops == 0 || num_frames == 0 || n_crops >= (1u << 30) ||
+        (mode != CLX_OUT_CHANNELS_I32 && mode != CLX_OUT_CHANNELS_F32) || (mode == CLX_OUT_CHANNELS_F32 && corpus->max_bps > 24))
+        return CLX_ERR_INVALID_ARGUMENT;
+    const size_t S = clx_crop_frames_bound(corpus->descs.data(), corpus->n_frames, corpus->file_frames.data(),
+                                           corpus->n_files, num_frames);
+    const size_t C = corpus->channels, rows = n_crops * C;  // (< 2^33: no overflow)
+    const clx::Plan plan = make_plan(ctx, corpus->descs.data(), corpus->descs.size());
+    const size_t slot_elems = ((size_t)plan.max_frame_elems + 3) & ~(size_t)3;
+    if (S == 0 || S > UINT32_MAX / n_crops || num_frames > (SIZE_MAX / 4 - 8) / (rows + C)) return CLX_ERR_INVALID_ARGUMENT;
+    const size_t slots = n_crops * S;
+    if (slots > (SIZE_MAX / 4 - 8) / slot_elems) return CLX_ERR_INVALID_ARGUMENT;
+    CU(ctx, cudaSetDevice(ctx->device));
+    clx_batch* b = new clx_batch();
+    b->corpus = corpus;
+    corpus->live++;
+    b->d_bytes = corpus->d_bytes;
+    b->nbytes = corpus->nbytes;
+    b->buf_bytes = corpus->buf_bytes;
+    b->n_frames = (uint32_t)slots;
+    b->out_elems = rows * num_frames;
+    b->plan = plan;
+    b->mode = mode;
+    b->stride = num_frames;
+    b->device_crc = !(ctx->flags & CLX_OPT_NO_VERIFY_CRC);
+    clx::CropBuffers& cb = b->crop;
+    cb.n_crops = (uint32_t)n_crops;
+    cb.C = (uint32_t)C;
+    cb.S = (uint32_t)S;
+    cb.n_slots = (uint32_t)slots;
+    cb.L = num_frames;
+    cb.slot_elems = slot_elems;
+    const size_t conv_elems = (rows + C) * num_frames + 8;  // the output, C trash rows for the unused slots, vector slack
+    cudaError_t e = cudaMalloc((void**)&b->d_descs, slots * sizeof(clx_frame_desc));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_out, (slots * slot_elems + 4) * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_results, slots * sizeof(clx_frame_result));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_need_hi, 4 * sizeof(int));
+    if (e == cudaSuccess) e = cudaMalloc(&b->d_params, clx::coop_params_bytes(plan, b->n_frames) + 16);
+    if (e == cudaSuccess) e = cudaMalloc(&b->d_conv, conv_elems * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMemset(b->d_conv, 0, conv_elems * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_mark, slots);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_cols, slots * sizeof(uint64_t));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_wins, slots * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.requests, n_crops * sizeof(clx_crop_request));
+    if (e == cudaSuccess) e = cudaMemset((void*)cb.requests, 0, n_crops * sizeof(clx_crop_request));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.status, n_crops * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMemset(cb.status, 0, n_crops * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.lengths, n_crops * sizeof(int64_t));
+    if (e == cudaSuccess) e = cudaMemset(cb.lengths, 0, n_crops * sizeof(int64_t));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.error, sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMemset(cb.error, 0xff, sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.plan, n_crops * sizeof(clx::CropPlan));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.scan, (n_crops + 1) * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
+    if (e != cudaSuccess) {
+        clx_batch_destroy(ctx, b);
+        return cuda_fail(ctx, e, "clx_batch_create_crops");
+    }
+    build_graph(ctx, b);
+    *out = b;
+    return CLX_OK;
+}
+
+void* clx_batch_crop_requests(clx_batch* b) { return b && b->corpus ? (void*)b->crop.requests : nullptr; }
+void* clx_batch_crop_status(clx_batch* b) { return b && b->corpus ? (void*)b->crop.status : nullptr; }
+void* clx_batch_crop_lengths(clx_batch* b) { return b && b->corpus ? (void*)b->crop.lengths : nullptr; }
+void* clx_batch_crop_error(clx_batch* b) { return b && b->corpus ? (void*)b->crop.error : nullptr; }
 
 }  // extern "C"
 

@@ -92,6 +92,43 @@ cudaError_t launch_channels(const clx_frame_desc* d_descs, uint32_t n_frames, ui
 // mark[f] = (results[f].status == status) for every frame, unless *gate == 0 (then nothing is written).
 cudaError_t launch_mark_status(const clx_frame_result* d_results, uint32_t n_frames, int32_t status, uint8_t* d_mark,
                                const int* gate, cudaStream_t stream, uint64_t* launches);
+// clx_crops.cu: crop batches.  A corpus on the device: its descriptors (descs[n_frames] is the filler frame), each
+// frame's first sample within its file, each file's frame range [file_frames[i], file_frames[i + 1]), length, channel
+// count and trailing-bytes verdict.
+struct CropCorpus {
+    const clx_frame_desc* descs;
+    const int64_t* starts;
+    const uint32_t* file_frames;
+    const int64_t* file_len;
+    const uint32_t* file_ch;
+    const int32_t* file_tail;
+    uint32_t n_files, n_frames;
+};
+// Per crop, what the planner found (device memory, written every decode).
+struct CropPlan {
+    int64_t lo;       // first sample of the excerpt
+    uint32_t count;   // frames overlapping it
+    uint32_t first;   // corpus index of the first of them
+    uint32_t file;
+    uint32_t ch;      // rows the excerpt covers (0: an invalid request)
+};
+struct CropBuffers {
+    const clx_crop_request* requests;
+    int32_t* status;
+    int64_t* lengths;
+    unsigned long long* error;
+    CropPlan* plan;
+    uint32_t* scan;   // n_crops + 1: exclusive scan of the counts, then the total
+    uint32_t n_crops, C, S, n_slots;
+    uint64_t L;       // num_frames: the row length
+    uint64_t slot_elems;
+};
+// Filler frame: 1 channel, 16 bits, block size 192, CONSTANT 0.  Writes it if cap suffices; returns its length.
+size_t filler_frame(uint8_t* out, size_t cap);
+// The crop batch's launch sequence: planner (count, scan, emit, zero-fill), launch_decode over every slot, status pass.
+// `db`: the batch's buffers; db.descs / db.cols / db.wins are written by the planner.
+cudaError_t launch_crops(const CropCorpus& cc, const CropBuffers& cb, const DecodeBuffers& db, const Plan& plan, bool crc,
+                         cudaStream_t stream, uint64_t* launches);
 #ifdef CLX_EXPERIMENT
 extern int g_exp_which;  // measurement builds only: bit 0 = index pass, bit 1 = decode pass of LanePerFrame
 extern int g_exp_dyn_smem;

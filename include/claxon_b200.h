@@ -267,6 +267,65 @@ typedef struct clx_frame_window {
 int clx_batch_create_windows(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
                              const clx_frame_window* windows, size_t n_frames, uint32_t n_rows, size_t row_stride,
                              uint32_t batch_flags, uint32_t mode, clx_batch** out);
+/* Device-resident corpora and crop batches: the frames of several FLAC streams uploaded once, and fixed-shape batches of
+ * [B, C, L] excerpts of them that plan each call's frames, windows and columns on the device, inside the batch's graph.
+ * A call is then: write the requests into clx_batch_crop_requests (device memory), clx_batch_decode; nothing is gathered,
+ * uploaded, checksummed or instantiated per call, and the offsets may come from device code.
+ *
+ * clx_corpus_create: `bytes` (host memory) holds the frames of n_files streams; file i's frames are descs[file_frames[i]
+ * .. file_frames[i + 1]) in stream order (file_frames has n_files + 1 entries), byte_offset indexing `bytes`; out_offset
+ * is ignored.  Sample t of file i is sample t - start of the frame that holds it, a frame's start being the sum of the
+ * block sizes before it in its file.  The bytes and descriptors are uploaded once, with each frame's start and each
+ * file's frame range and length.  A file whose last frame lacks CLX_FRAME_CRC16_VERIFIED (its end is unconfirmed) has
+ * that frame decoded once here: if it decodes and ends before its byte_len, the frame header status at its end (other
+ * than CLX_EOF) is the file's trailing-bytes verdict, reported by every crop that contains that frame.
+ * CLX_ERR_INVALID_ARGUMENT for: every descriptor condition of the create calls above, file_frames not monotone or not
+ * ending at n_frames, frames of one file with different channel counts, n_frames or n_files of 2^32 - 1 or more.
+ * clx_corpus_destroy: CLX_ERR_INVALID_ARGUMENT (and nothing freed) while a crop batch of the corpus is alive. */
+typedef struct clx_corpus clx_corpus;
+int clx_corpus_create(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
+                      const uint32_t* file_frames, size_t n_files, clx_corpus** out);
+int clx_corpus_destroy(clx_ctx* ctx, clx_corpus* corpus);
+/* The most frames that can overlap num_frames consecutive samples of one file: with m the smallest block size among the
+ * frames that are not the last of their file, floor((num_frames - 2) / m) + 2 for num_frames >= 2 and 1 for num_frames
+ * 1, but never more than the frames of the largest file (and 1 when no file has two frames).  Host only.  0 for
+ * num_frames 0 or a bad file_frames. */
+size_t clx_crop_frames_bound(const clx_frame_desc* descs, size_t n_frames, const uint32_t* file_frames, size_t n_files,
+                             size_t num_frames);
+/* A crop batch of n_crops excerpts of num_frames samples each, in mode CLX_OUT_CHANNELS_I32 or _F32.  It is an ordinary
+ * clx_batch (clx_batch_decode, _sync, _last_kernel_ms, _read_to, clx_ctx_run_steps, clx_batch_device_out work on it)
+ * that shares the corpus's bytes.  Output: [n_crops * C, num_frames] channels-first, C the corpus's largest channel
+ * count; crop b is rows [b * C, (b + 1) * C).  Each decode reads request b = {file, reserved, offset}: samples [offset,
+ * min(offset + num_frames, length)) of that file go to row b * C + c, columns from 0; every other element of the crop's
+ * rows is 0.  A request with file >= n_files, reserved != 0, offset < 0 or offset > length gets status
+ * CLX_ERR_INVALID_ARGUMENT, length 0 and zero rows.  Status of a valid crop: the first failed frame in stream order,
+ * else the file's trailing-bytes verdict when the crop contains its last frame, else CLX_OK; a failed crop's rows are
+ * unspecified.  The frame CRC-16 is checked on the device in every decode (frames the demuxer confirmed are skipped).
+ * F32 is refused when ANY frame of the corpus has more than 24 bits, since the batch may be asked for any of them.
+ * Memory: (n_crops + 1) * C * num_frames output elements (the C rows after the output take the unused slots) and, per
+ * slot, a planar scratch of the corpus's largest frame; slots = n_crops * clx_crop_frames_bound(num_frames).
+ * CLX_ERR_INVALID_ARGUMENT for: n_crops or num_frames 0, n_crops of 2^30 or more, slots of 2^32 or more, sizes that
+ * overflow, a mode other than the two channels modes, F32 with a frame above 24 bits. */
+typedef struct clx_crop_request {
+    uint32_t file;     /* index of the file in the corpus */
+    uint32_t reserved; /* 0 */
+    int64_t offset;    /* first sample of the excerpt, 0 .. the file's length */
+} clx_crop_request;
+int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, size_t num_frames, uint32_t mode,
+                           clx_batch** out);
+/* Device pointers of a crop batch (NULL for other batches).  requests: n_crops clx_crop_request, written by the caller
+ * before clx_batch_decode (zeroed at creation).  status: n_crops int32.  lengths: n_crops int64, min(num_frames,
+ * length - offset), 0 for an invalid request.  error: one uint64, ~0 when every crop is CLX_OK, else the failure a
+ * caller checking the whole batch reports first: (kind << 62) | (crop << 32) | (uint32_t)status, kind 0 an invalid
+ * request, 1 a failed frame, 2 a trailing-bytes verdict; the smallest such value, so invalid requests before failed
+ * frames before trailing bytes, each in crop order. */
+void* clx_batch_crop_requests(clx_batch* b);
+void* clx_batch_crop_status(clx_batch* b);
+void* clx_batch_crop_lengths(clx_batch* b);
+void* clx_batch_crop_error(clx_batch* b);
+/* The frame a crop batch decodes in its unused slots (1 channel, 16 bits, 192 samples of CONSTANT 0, valid CRC-8 and
+ * CRC-16), for inspection: writes it into out if cap suffices and returns its length in bytes.  Host only. */
+size_t clx_crop_filler_frame(uint8_t* out, size_t cap);
 int clx_batch_decode(clx_ctx* ctx, clx_batch* b, uint32_t stream_index); /* async on an internal stream */
 int clx_batch_sync(clx_ctx* ctx, clx_batch* b);
 /* Planar batches only (CLX_ERR_INVALID_ARGUMENT for any other mode). */

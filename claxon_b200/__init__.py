@@ -939,13 +939,22 @@ class _DeviceView:
 
 
 class Corpus:
-    """The compressed frames of a FlacIndex's files, uploaded to the GPU once with their frame index
-    (clx_corpus_create), for CropBatch: crops whose frames, windows and columns are planned on the device.  Each file's
-    bytes from its first frame to its end are uploaded; the trailing-bytes verdict of a file whose last frame's end is
-    unconfirmed is taken once here.  `index` is kept for error messages."""
+    """The compressed frames of a FlacIndex's files, copied once with their frame index (clx_corpus_create_ex), for
+    CropBatch: crops whose frames, windows and columns are planned on the device.  Each file's bytes from its first
+    frame to its end are copied; the trailing-bytes verdict of a file whose last frame's end is unconfirmed is taken
+    once here.  `index` is kept for error messages.
 
-    def __init__(self, index: FlacIndex, ctx: Context | None = None):
+    `memory`: where the bytes live.  "device" (the default) uploads them to the GPU.  "host" keeps them in pinned host
+    memory the GPU reads directly, and only the frame index (about 48 bytes per frame) on the GPU: for corpora that
+    should not take GPU memory from the model.  Every call of a crop batch of a host corpus then copies the frames its
+    crops selected over PCIe first (about the crops' span bytes x B per call), so it is slower than over a device
+    corpus; the results are the same.  `device_bytes` is the GPU memory the corpus holds."""
+
+    def __init__(self, index: FlacIndex, ctx: Context | None = None, memory: str = "device"):
+        if memory not in ("device", "host"):
+            raise ValueError('memory must be "device" or "host"')
         self.index = index
+        self.memory = memory
         self.ctx = ctx or default_context()
         chunks, parts, file_frames, at = [], [], [0], 0
         for f in index.files:
@@ -964,21 +973,35 @@ class Corpus:
         self.nbytes = int(data.size)
         self.channels = max([int(self.descs["n_channels"].max())] if self.descs.size else [1])
         h = C.c_void_p()
-        _check(self.ctx._L.clx_corpus_create(self.ctx._h, data.ctypes.data, data.size, self.descs.ctypes.data,
-                                             self.descs.size, self.file_frames.ctypes.data, len(index), C.byref(h)), self.ctx)
+        flags = _lib.CORPUS_HOST if memory == "host" else 0
+        _check(self.ctx._L.clx_corpus_create_ex(self.ctx._h, data.ctypes.data, data.size, self.descs.ctypes.data,
+                                                self.descs.size, self.file_frames.ctypes.data, len(index), flags,
+                                                C.byref(h)), self.ctx)
         self._h = h
+
+    @property
+    def device_bytes(self) -> int:
+        """clx_corpus_device_bytes: the GPU memory the corpus holds (its bytes too for a device corpus)."""
+        return int(self.ctx._L.clx_corpus_device_bytes(self._h))
 
     def frames_bound(self, num_frames: int) -> int:
         """clx_crop_frames_bound: the most frames num_frames consecutive samples of one file can overlap."""
         return int(self.ctx._L.clx_crop_frames_bound(self.descs.ctypes.data, self.descs.size, self.file_frames.ctypes.data,
                                                      len(self.index), int(num_frames)))
 
+    def bytes_bound(self, num_frames: int) -> int:
+        """clx_crop_bytes_bound: the most compressed bytes a crop of num_frames samples can span."""
+        return int(self.ctx._L.clx_crop_bytes_bound(self.descs.ctypes.data, self.descs.size, self.file_frames.ctypes.data,
+                                                    len(self.index), int(num_frames)))
+
     def crops(self, batch: int, num_frames: int, dtype=None) -> "CropBatch":
-        """A CropBatch of `batch` crops of `num_frames` samples; its CUDA graph is instantiated here."""
+        """A CropBatch of `batch` crops of `num_frames` samples; its CUDA graph is instantiated here.  Over a host
+        corpus, the batch also holds a GPU staging buffer of about batch x bytes_bound(num_frames) bytes, and each call
+        reads the selected crops' span bytes (about span bytes x batch) from host memory over PCIe."""
         return CropBatch(self, batch, num_frames, dtype)
 
     def close(self):
-        """Frees the device copy; raises Error while a CropBatch of the corpus is alive."""
+        """Frees the corpus's copy of the bytes and its index; raises Error while a CropBatch of the corpus is alive."""
         if getattr(self, "_h", None) and getattr(self.ctx, "_h", None):
             _check(self.ctx._L.clx_corpus_destroy(self.ctx._h, self._h), self.ctx)
         self._h = None
@@ -1019,7 +1042,11 @@ class CropBatch:
     (and `status`, an int32 CUDA tensor of per-crop statuses) are views of the batch's own buffers, overwritten by the
     next call; the next call waits for what torch's current stream has enqueued before it, so reading them on that stream
     is safe, clone() them to keep them.  Unlike load_crops(), a float32 batch is refused when any frame of the corpus
-    has more than 24 bits (load_crops() refuses only the frames a call selects)."""
+    has more than 24 bits (load_crops() refuses only the frames a call selects).
+
+    Over a host corpus (Corpus(memory="host")), each call first copies every crop's span of frames from pinned host
+    memory into a GPU staging buffer, one more kernel in the graph: about span bytes x B cross PCIe per call.  Results
+    are the same as over a device corpus."""
 
     def __init__(self, corpus: Corpus, batch: int, num_frames: int, dtype=None):
         import torch

@@ -53,6 +53,7 @@ OPT_NO_GENERIC = 16
 OPT_NO_WIDE = 32
 OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT = 1, 2
 BATCH_BYTES_ON_DEVICE = 1
+CORPUS_HOST = 1
 OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24 = 0, 1, 2, 3
 OUT_CHANNELS_I32, OUT_CHANNELS_F32 = 4, 5
 FRAME_VARIABLE_BLOCKING = 1
@@ -90,8 +91,11 @@ SYMBOLS = {
     "clx_batch_create_windows": (C.c_int, [_vp, _u8p, _sz, _vp, _vp, _sz, C.c_uint32, _sz, C.c_uint32, C.c_uint32,
                                            C.POINTER(_vp)]),
     "clx_corpus_create": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _vp, _sz, C.POINTER(_vp)]),
+    "clx_corpus_create_ex": (C.c_int, [_vp, _u8p, _sz, _vp, _sz, _vp, _sz, C.c_uint32, C.POINTER(_vp)]),
     "clx_corpus_destroy": (C.c_int, [_vp, _vp]),
+    "clx_corpus_device_bytes": (_sz, [_vp]),
     "clx_crop_frames_bound": (_sz, [_vp, _sz, _vp, _sz, _sz]),
+    "clx_crop_bytes_bound": (_sz, [_vp, _sz, _vp, _sz, _sz]),
     "clx_batch_create_crops": (C.c_int, [_vp, _vp, _sz, _sz, C.c_uint32, C.POINTER(_vp)]),
     "clx_batch_crop_requests": (_vp, [_vp]),
     "clx_batch_crop_status": (_vp, [_vp]),

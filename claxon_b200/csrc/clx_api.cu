@@ -151,13 +151,18 @@ struct clx_batch {
     uint32_t* d_wins = nullptr;
     uint64_t stride = 0;
     // Crop batches (clx_batch_create_crops): d_bytes is the corpus's, not the batch's; the planner writes d_descs,
-    // d_cols and d_wins in every decode (clx_crops.cu).
+    // d_cols and d_wins in every decode (clx_crops.cu).  Over a host corpus, d_bytes is the batch's own staging buffer:
+    // n_crops spans of span_stride bytes, then the filler frame.
     clx_corpus* corpus = nullptr;
     clx::CropBuffers crop{};
+    uint64_t span_stride = 0;
 };
 
 struct clx_corpus {
     uint8_t* d_bytes = nullptr; size_t nbytes = 0, buf_bytes = 0;
+    uint8_t* h_bytes = nullptr;        // CLX_CORPUS_HOST: the bytes in mapped pinned memory (then d_bytes is null)
+    const uint8_t* d_host = nullptr;   // ... and their device address
+    size_t device_bytes = 0;           // every device allocation of the corpus
     clx_frame_desc* d_descs = nullptr;  // n_frames + 1: the filler frame last
     int64_t* d_starts = nullptr;
     uint32_t* d_file_frames = nullptr;
@@ -169,8 +174,9 @@ struct clx_corpus {
     std::vector<uint32_t> file_frames;
     uint32_t channels = 1, max_bps = 0;
     int live = 0;  // crop batches of this corpus
-    clx::CropCorpus view() const {
-        return {d_descs, d_starts, d_file_frames, d_file_len, d_file_ch, d_file_tail, n_files, n_frames};
+    clx::CropCorpus view(uint64_t span_stride) const {
+        return {d_descs, d_starts, d_file_frames, d_file_len, d_file_ch, d_file_tail, n_files, n_frames, d_host,
+                d_host ? span_stride : 0};
     }
 };
 
@@ -629,7 +635,8 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
     const clx::DecodeBuffers db{b->d_bytes, b->buf_bytes, b->d_descs, b->n_frames, b->d_out, b->d_results, b->d_need_hi,
                                 b->d_params, b->mode, b->d_conv, b->d_mark, b->d_cols, b->stride, b->d_wins};
-    if (b->corpus) return clx::launch_crops(b->corpus->view(), b->crop, db, b->plan, b->device_crc, st, launches);
+    if (b->corpus)
+        return clx::launch_crops(b->corpus->view(b->span_stride), b->crop, db, b->plan, b->device_crc, st, launches);
     return clx::launch_decode(db, b->plan, b->device_crc, st, launches);
 }
 
@@ -756,7 +763,8 @@ int clx_batch_read_to(clx_ctx* ctx, clx_batch* b, void* out, size_t out_elems, c
 void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
     (void)ctx;
     if (!b) return;
-    if (b->corpus) {  // the bytes are the corpus's
+    if (b->corpus) {  // the bytes are the corpus's, or over a host corpus the batch's staging buffer
+        if (b->corpus->h_bytes) cudaFree(b->d_bytes);
         b->corpus->live--;
         cudaFree((void*)b->crop.requests); cudaFree(b->crop.status); cudaFree(b->crop.lengths); cudaFree(b->crop.error);
         cudaFree(b->crop.plan); cudaFree(b->crop.scan);
@@ -835,6 +843,7 @@ namespace {
 void free_corpus(clx_corpus* c) {
     cudaFree(c->d_bytes); cudaFree(c->d_descs); cudaFree(c->d_starts); cudaFree(c->d_file_frames);
     cudaFree(c->d_file_len); cudaFree(c->d_file_ch); cudaFree(c->d_file_tail);
+    if (c->h_bytes) cudaFreeHost(c->h_bytes);
     delete c;
 }
 
@@ -861,8 +870,15 @@ extern "C" {
 
 int clx_corpus_create(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
                       const uint32_t* file_frames, size_t n_files, clx_corpus** out) {
+    return clx_corpus_create_ex(ctx, bytes, nbytes, descs, n_frames, file_frames, n_files, 0, out);
+}
+
+int clx_corpus_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
+                         const uint32_t* file_frames, size_t n_files, uint32_t flags, clx_corpus** out) {
     if (!ctx || !out || (!bytes && nbytes) || (!descs && n_frames) || !file_frames) return CLX_ERR_INVALID_ARGUMENT;
     *out = nullptr;
+    if (flags & ~CLX_CORPUS_HOST) return CLX_ERR_INVALID_ARGUMENT;
+    const bool host = flags & CLX_CORPUS_HOST;
     if (n_frames >= UINT32_MAX || n_files >= UINT32_MAX || file_frames[n_files] != n_frames) return CLX_ERR_INVALID_ARGUMENT;
     for (size_t i = 0; i < n_files; i++)
         if (file_frames[i + 1] < file_frames[i]) return CLX_ERR_INVALID_ARGUMENT;
@@ -871,6 +887,12 @@ int clx_corpus_create(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const c
         at0.out_offset = 0;
         if (!valid_desc(at0, nbytes, (size_t)descs[i].n_channels * descs[i].block_size)) return CLX_ERR_INVALID_ARGUMENT;
     }
+    // A host corpus gathers a crop's frames as one span from its first frame's start to its last frame's end.
+    for (size_t i = 0; host && i < n_files; i++)
+        for (size_t f = file_frames[i] + 1; f < file_frames[i + 1]; f++)
+            if (descs[f].byte_offset < descs[f - 1].byte_offset ||
+                descs[f].byte_offset + descs[f].byte_len < descs[f - 1].byte_offset + descs[f - 1].byte_len)
+                return CLX_ERR_INVALID_ARGUMENT;
     CU(ctx, cudaSetDevice(ctx->device));
     clx_corpus* c = new clx_corpus();
     c->n_frames = (uint32_t)n_frames;
@@ -914,12 +936,26 @@ int clx_corpus_create(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const c
     fd.out_offset = 0;
     c->descs.push_back(fd);
     c->buf_bytes = ((nbytes + filler_len + 63) & ~(size_t)63) + 128;  // whole 64-byte TMA chunks + look-ahead
-    cudaError_t e = cudaMalloc((void**)&c->d_bytes, c->buf_bytes);
-    if (e == cudaSuccess) e = cudaMemset(c->d_bytes, 0, c->buf_bytes);
-    if (e == cudaSuccess && nbytes) e = cudaMemcpy(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(c->d_bytes + nbytes, filler, filler_len, cudaMemcpyHostToDevice);
+    cudaError_t e = cudaSuccess;
+    if (host) {  // the crop batches stage what they decode; the filler frame is copied from here into each of them
+        e = cudaHostAlloc((void**)&c->h_bytes, c->buf_bytes, cudaHostAllocMapped);
+        if (e == cudaSuccess) {
+            memset(c->h_bytes, 0, c->buf_bytes);
+            if (nbytes) memcpy(c->h_bytes, bytes, nbytes);
+            memcpy(c->h_bytes + nbytes, filler, filler_len);
+            e = cudaHostGetDevicePointer((void**)&c->d_host, c->h_bytes, 0);
+        }
+    } else {
+        e = cudaMalloc((void**)&c->d_bytes, c->buf_bytes);
+        if (e == cudaSuccess) c->device_bytes += c->buf_bytes;
+        if (e == cudaSuccess) e = cudaMemset(c->d_bytes, 0, c->buf_bytes);
+        if (e == cudaSuccess && nbytes) e = cudaMemcpy(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) e = cudaMemcpy(c->d_bytes + nbytes, filler, filler_len, cudaMemcpyHostToDevice);
+    }
     auto put = [&](auto*& dst, const auto& v) {
-        if (e == cudaSuccess) e = cudaMalloc((void**)&dst, std::max<size_t>(1, v.size()) * sizeof(v[0]));
+        const size_t size = std::max<size_t>(1, v.size()) * sizeof(v[0]);
+        if (e == cudaSuccess) e = cudaMalloc((void**)&dst, size);
+        if (e == cudaSuccess) c->device_bytes += size;
         if (e == cudaSuccess && !v.empty()) e = cudaMemcpy(dst, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice);
     };
     put(c->d_descs, c->descs);
@@ -944,6 +980,8 @@ int clx_corpus_destroy(clx_ctx* ctx, clx_corpus* corpus) {
     return CLX_OK;
 }
 
+size_t clx_corpus_device_bytes(const clx_corpus* corpus) { return corpus ? corpus->device_bytes : 0; }
+
 int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, size_t num_frames, uint32_t mode,
                            clx_batch** out) {
     if (!out) return CLX_ERR_INVALID_ARGUMENT;
@@ -959,6 +997,17 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
     if (S == 0 || S > UINT32_MAX / n_crops || num_frames > (SIZE_MAX / 4 - 8) / (rows + C)) return CLX_ERR_INVALID_ARGUMENT;
     const size_t slots = n_crops * S;
     if (slots > (SIZE_MAX / 4 - 8) / slot_elems) return CLX_ERR_INVALID_ARGUMENT;
+    // Over a host corpus: crop b's span at b * span_stride + (its start & 15), the filler frame after the last span,
+    // then whole 64-byte TMA chunks + look-ahead (DecodeBuffers' contract).
+    size_t span_stride = 0, staging = 0;
+    const size_t filler_len = clx::filler_frame(nullptr, 0);
+    if (corpus->h_bytes) {
+        const size_t span = clx_crop_bytes_bound(corpus->descs.data(), corpus->n_frames, corpus->file_frames.data(),
+                                                 corpus->n_files, num_frames);
+        span_stride = (span + 15 + 15) & ~(size_t)15;
+        if (span_stride > (SIZE_MAX / 2) / n_crops) return CLX_ERR_INVALID_ARGUMENT;
+        staging = ((n_crops * span_stride + filler_len + 63) & ~(size_t)63) + 128;
+    }
     CU(ctx, cudaSetDevice(ctx->device));
     clx_batch* b = new clx_batch();
     b->corpus = corpus;
@@ -966,6 +1015,17 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
     b->d_bytes = corpus->d_bytes;
     b->nbytes = corpus->nbytes;
     b->buf_bytes = corpus->buf_bytes;
+    b->span_stride = span_stride;
+    cudaError_t e = cudaSuccess;
+    if (corpus->h_bytes) {
+        b->nbytes = n_crops * span_stride + filler_len;
+        b->buf_bytes = staging;
+        e = cudaMalloc((void**)&b->d_bytes, staging);
+        if (e == cudaSuccess) e = cudaMemset(b->d_bytes, 0, staging);
+        if (e == cudaSuccess)
+            e = cudaMemcpy(b->d_bytes + n_crops * span_stride, corpus->h_bytes + corpus->nbytes, filler_len,
+                           cudaMemcpyHostToDevice);
+    }
     b->n_frames = (uint32_t)slots;
     b->out_elems = rows * num_frames;
     b->plan = plan;
@@ -980,7 +1040,7 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
     cb.L = num_frames;
     cb.slot_elems = slot_elems;
     const size_t conv_elems = (rows + C) * num_frames + 8;  // the output, C trash rows for the unused slots, vector slack
-    cudaError_t e = cudaMalloc((void**)&b->d_descs, slots * sizeof(clx_frame_desc));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_descs, slots * sizeof(clx_frame_desc));
     if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_out, (slots * slot_elems + 4) * sizeof(int32_t));
     if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_results, slots * sizeof(clx_frame_result));
     if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_need_hi, 4 * sizeof(int));

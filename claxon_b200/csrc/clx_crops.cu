@@ -1,15 +1,18 @@
-// clx_crops.cu — crop batches (include/claxon_b200.h, clx_batch_create_crops): [B, C, L] excerpts of a device-resident
-// corpus, planned on the device inside the batch's graph.
+// clx_crops.cu — crop batches (include/claxon_b200.h, clx_batch_create_crops): [B, C, L] excerpts of a corpus in device
+// or pinned host memory, planned on the device inside the batch's graph.
 //
 // The graph: the planner, then clx::launch_decode over every slot (with the device CRC-16), then the status pass.
 //   1. crop_count_kernel: per crop, validate the request and binary-search the file's frame starts for the frames that
 //      overlap [offset, min(offset + L, length)) (plan_range in claxon_b200/__init__.py does the same on the host).
 //   2. crop_scan_kernel: one CTA, exclusive scan of the counts, so crops take consecutive slots in crop order and frames
 //      in stream order (the device order of load_crops()'s windowed batch on a corpus of one shape).
-//   3. crop_emit_kernel: per slot, the frame's descriptor (out_offset = its place in the planar scratch), its column on
-//      the crop's first row and its window.  Slots past the total go to the C trash rows after the output: up to the
-//      next multiple of 32 they repeat the last planned frame, after that they get the filler frame, so fillers share
-//      warps only with each other; no window has count 0.
+//   2b. crop_gather_kernel, host corpora only: copies each crop's span of consecutive frames from mapped host memory
+//      into its span of the batch's staging buffer, the layout load_crops() gathers on the host.
+//   3. crop_emit_kernel: per slot, the frame's descriptor (out_offset = its place in the planar scratch; over a host
+//      corpus, byte_offset = its place in the staging buffer), its column on the crop's first row and its window.  Slots
+//      past the total go to the C trash rows after the output: up to the next multiple of 32 they repeat the last
+//      planned frame, after that they get the filler frame, so fillers share warps only with each other; no window has
+//      count 0.
 //   4. crop_zero_kernel: zeroes exactly what no window of this call covers (columns past each crop's length, rows a
 //      file does not have, every row of an invalid crop); the output is never cleared as a whole.
 //   5. crop_status_kernel, after the decode: per crop the first failed slot, else the trailing-bytes verdict.
@@ -110,6 +113,46 @@ crop_scan_kernel(const CropPlan* __restrict__ plan, uint32_t n, uint32_t* __rest
     if (threadIdx.x == 0) scan[n] = s_carry;
 }
 
+// Every load is a PCIe round trip of the order of a microsecond, so the grid keeps many in flight: a CTA copies
+// GATHER_CHUNK bytes of one crop's span, each thread GATHER_VECS independent 16-byte loads before its stores.
+constexpr uint32_t GATHER_THREADS = 256;
+constexpr uint32_t GATHER_VECS = 4;
+constexpr uint64_t GATHER_CHUNK = (uint64_t)GATHER_THREADS * GATHER_VECS * 16;
+
+// Grid: x over the chunks of a span, y over the crops.  Crop b's span [byte_offset(first), byte_offset(last) +
+// byte_len(last)) goes to staging + b * span_stride + (start & 15): source and destination agree mod 16, so the body is
+// 16-byte vectors between a scalar head and tail.  Crops without frames copy nothing.
+__global__ void __launch_bounds__(GATHER_THREADS)
+crop_gather_kernel(CropCorpus cc, CropBuffers cb, uint8_t* __restrict__ staging) {
+    for (uint32_t b = blockIdx.y; b < cb.n_crops; b += gridDim.y) {
+        const CropPlan p = cb.plan[b];
+        if (p.count == 0) continue;
+        const uint64_t s0 = cc.descs[p.first].byte_offset;
+        const clx_frame_desc& last = cc.descs[p.first + p.count - 1];
+        const uint64_t s1 = last.byte_offset + last.byte_len;
+        const uint64_t delta = (uint64_t)b * cc.span_stride + (s0 & 15) - s0;  // source byte x goes to staging[x + delta]
+        uint64_t a = (s0 + 15) & ~(uint64_t)15, e = s1 & ~(uint64_t)15;      // the vector part [a, e)
+        if (e < a) a = e = s1;                                                // within one 16-byte block: all head
+        if (blockIdx.x == 0 && threadIdx.x < 32) {  // head [s0, a) on threads 0-15, tail [e, s1) on 16-31
+            const uint64_t x = threadIdx.x < 16 ? s0 + threadIdx.x : e + (threadIdx.x - 16);
+            if (x < (threadIdx.x < 16 ? a : s1)) staging[x + delta] = cc.host_bytes[x];
+        }
+        const uint4* src = reinterpret_cast<const uint4*>(cc.host_bytes + a);
+        uint4* dst = reinterpret_cast<uint4*>(staging + (a + delta));
+        const uint64_t n = (e - a) >> 4;
+        for (uint64_t v = (uint64_t)blockIdx.x * GATHER_THREADS * GATHER_VECS + threadIdx.x; v < n;
+             v += (uint64_t)gridDim.x * GATHER_THREADS * GATHER_VECS) {
+            uint4 r[GATHER_VECS];
+#pragma unroll
+            for (uint32_t j = 0; j < GATHER_VECS; j++)
+                if (v + j * GATHER_THREADS < n) r[j] = src[v + j * GATHER_THREADS];
+#pragma unroll
+            for (uint32_t j = 0; j < GATHER_VECS; j++)
+                if (v + j * GATHER_THREADS < n) dst[v + j * GATHER_THREADS] = r[j];
+        }
+    }
+}
+
 __global__ void __launch_bounds__(CROP_THREADS)
 crop_emit_kernel(CropCorpus cc, CropBuffers cb, clx_frame_desc* __restrict__ descs, uint64_t* __restrict__ cols,
                  uint32_t* __restrict__ wins) {
@@ -126,6 +169,7 @@ crop_emit_kernel(CropCorpus cc, CropBuffers cb, clx_frame_desc* __restrict__ des
     const uint32_t slot = s < total ? s : s < ((total + 31) & ~31u) ? total - 1 : UINT32_MAX;
     if (slot == UINT32_MAX) {
         d = cc.descs[cc.n_frames];
+        if (cc.span_stride) d.byte_offset = (uint64_t)cb.n_crops * cc.span_stride;  // staged after the spans at creation
     } else {
         // the crop that owns the slot: the last b with scan[b] <= slot (crops without frames own no slot)
         uint32_t a = 0, e = cb.n_crops;
@@ -138,6 +182,10 @@ crop_emit_kernel(CropCorpus cc, CropBuffers cb, clx_frame_desc* __restrict__ des
         const CropPlan p = cb.plan[b];
         const uint32_t f = p.first + (slot - cb.scan[b]);
         d = cc.descs[f];
+        if (cc.span_stride) {  // where crop_gather_kernel put the frame: its crop's span base plus its place in the span
+            const uint64_t b0 = cc.descs[p.first].byte_offset;
+            d.byte_offset = (uint64_t)b * cc.span_stride + (b0 & 15) + (d.byte_offset - b0);
+        }
         const int64_t s0 = cc.starts[f], hi = p.lo + cb.lengths[b];
         const int64_t first = max(p.lo - s0, (int64_t)0);
         const int64_t count = min(s0 + (int64_t)d.block_size, hi) - s0 - first;
@@ -197,6 +245,12 @@ cudaError_t launch_crops(const CropCorpus& cc, const CropBuffers& cb, const Deco
     const uint32_t crop_ctas = (cb.n_crops + CROP_THREADS - 1) / CROP_THREADS;
     crop_count_kernel<<<crop_ctas, CROP_THREADS, 0, stream>>>(cc, cb);
     crop_scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(cb.plan, cb.n_crops, cb.scan);
+    if (cc.host_bytes) {
+        const dim3 ggrid((uint32_t)std::min<uint64_t>((cc.span_stride + GATHER_CHUNK - 1) / GATHER_CHUNK, 65535),
+                         std::min<uint32_t>(cb.n_crops, 65535));
+        crop_gather_kernel<<<ggrid, GATHER_THREADS, 0, stream>>>(cc, cb, const_cast<uint8_t*>(db.bytes));
+        (*launches)++;
+    }
     crop_emit_kernel<<<(cb.n_slots + CROP_THREADS - 1) / CROP_THREADS, CROP_THREADS, 0, stream>>>(
         cc, cb, const_cast<clx_frame_desc*>(db.descs), const_cast<uint64_t*>(db.cols), const_cast<uint32_t*>(db.wins));
     const uint64_t rows = (uint64_t)cb.n_crops * cb.C;
@@ -247,6 +301,20 @@ size_t clx_crop_frames_bound(const clx_frame_desc* descs, size_t n_frames, const
     // k overlapping frames: the first and the last give at least one sample each, the k - 2 between them whole blocks
     const size_t s = (num_frames - 2) / m + 2;
     return std::max<size_t>(1, std::min(s, most));
+}
+
+size_t clx_crop_bytes_bound(const clx_frame_desc* descs, size_t n_frames, const uint32_t* file_frames, size_t n_files,
+                            size_t num_frames) {
+    const size_t S = clx_crop_frames_bound(descs, n_frames, file_frames, n_files, num_frames);
+    if (S == 0) return 0;
+    uint64_t most = 0;
+    for (size_t i = 0; i < n_files; i++)  // a crop from frame f spans f .. min(f + S, end of its file) - 1
+        for (size_t f = file_frames[i]; f < file_frames[i + 1]; f++) {
+            const clx_frame_desc& last = descs[std::min<size_t>(f + S, file_frames[i + 1]) - 1];
+            const uint64_t end = last.byte_offset + last.byte_len;
+            if (end > descs[f].byte_offset) most = std::max<uint64_t>(most, end - descs[f].byte_offset);
+        }
+    return most;
 }
 
 }  // extern "C"

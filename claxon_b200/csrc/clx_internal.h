@@ -94,7 +94,9 @@ cudaError_t launch_mark_status(const clx_frame_result* d_results, uint32_t n_fra
                                const int* gate, cudaStream_t stream, uint64_t* launches);
 // clx_crops.cu: crop batches.  A corpus on the device: its descriptors (descs[n_frames] is the filler frame), each
 // frame's first sample within its file, each file's frame range [file_frames[i], file_frames[i + 1]), length, channel
-// count and trailing-bytes verdict.
+// count and trailing-bytes verdict.  A corpus in host memory (CLX_CORPUS_HOST) also gives the device address of its
+// mapped pinned bytes and the batch's span stride: each call gathers crop b's span of frames into the batch's staging
+// buffer at b * span_stride + (span start & 15), and the descriptors point there.  Both are 0 for a device corpus.
 struct CropCorpus {
     const clx_frame_desc* descs;
     const int64_t* starts;
@@ -103,6 +105,8 @@ struct CropCorpus {
     const uint32_t* file_ch;
     const int32_t* file_tail;
     uint32_t n_files, n_frames;
+    const uint8_t* host_bytes;
+    uint64_t span_stride;
 };
 // Per crop, what the planner found (device memory, written every decode).
 struct CropPlan {
@@ -125,8 +129,9 @@ struct CropBuffers {
 };
 // Filler frame: 1 channel, 16 bits, block size 192, CONSTANT 0.  Writes it if cap suffices; returns its length.
 size_t filler_frame(uint8_t* out, size_t cap);
-// The crop batch's launch sequence: planner (count, scan, emit, zero-fill), launch_decode over every slot, status pass.
-// `db`: the batch's buffers; db.descs / db.cols / db.wins are written by the planner.
+// The crop batch's launch sequence: planner (count, scan, the gather of a host corpus, emit, zero-fill), launch_decode
+// over every slot, status pass.  `db`: the batch's buffers; db.descs / db.cols / db.wins are written by the planner, and
+// over a host corpus db.bytes is the staging buffer the gather writes.
 cudaError_t launch_crops(const CropCorpus& cc, const CropBuffers& cb, const DecodeBuffers& db, const Plan& plan, bool crc,
                          cudaStream_t stream, uint64_t* launches);
 #ifdef CLX_EXPERIMENT

@@ -281,17 +281,35 @@ int clx_batch_create_windows(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, 
  * than CLX_EOF) is the file's trailing-bytes verdict, reported by every crop that contains that frame.
  * CLX_ERR_INVALID_ARGUMENT for: every descriptor condition of the create calls above, file_frames not monotone or not
  * ending at n_frames, frames of one file with different channel counts, n_frames or n_files of 2^32 - 1 or more.
- * clx_corpus_destroy: CLX_ERR_INVALID_ARGUMENT (and nothing freed) while a crop batch of the corpus is alive. */
+ * clx_corpus_destroy: CLX_ERR_INVALID_ARGUMENT (and nothing freed) while a crop batch of the corpus is alive.
+ *
+ * clx_corpus_create_ex: clx_corpus_create with `flags`; 0 is clx_corpus_create.  CLX_CORPUS_HOST keeps the bytes in
+ * mapped pinned host memory instead of device memory (host RAM holds them once more, device memory only the frame
+ * index: descriptors, starts and the per-file arrays).  Each decode of a crop batch of such a corpus then copies the
+ * frames its crops selected over PCIe into a staging buffer of the batch (one more kernel in its graph) and decodes
+ * them there, with the same results.  A host corpus also needs each file's frames in byte order: byte_offset and
+ * byte_offset + byte_len non-decreasing within a file (as the demuxer gives them).  CLX_ERR_INVALID_ARGUMENT for
+ * unknown flag bits and, with CLX_CORPUS_HOST, frames out of byte order; otherwise as clx_corpus_create.
+ * clx_corpus_device_bytes: the device memory the corpus holds (its bytes for a device corpus, plus the frame index). */
+#define CLX_CORPUS_HOST 1u
 typedef struct clx_corpus clx_corpus;
 int clx_corpus_create(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
                       const uint32_t* file_frames, size_t n_files, clx_corpus** out);
+int clx_corpus_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
+                         const uint32_t* file_frames, size_t n_files, uint32_t flags, clx_corpus** out);
 int clx_corpus_destroy(clx_ctx* ctx, clx_corpus* corpus);
+size_t clx_corpus_device_bytes(const clx_corpus* corpus);
 /* The most frames that can overlap num_frames consecutive samples of one file: with m the smallest block size among the
  * frames that are not the last of their file, floor((num_frames - 2) / m) + 2 for num_frames >= 2 and 1 for num_frames
  * 1, but never more than the frames of the largest file (and 1 when no file has two frames).  Host only.  0 for
  * num_frames 0 or a bad file_frames. */
 size_t clx_crop_frames_bound(const clx_frame_desc* descs, size_t n_frames, const uint32_t* file_frames, size_t n_files,
                              size_t num_frames);
+/* The most compressed bytes one crop of num_frames samples can span: with S = clx_crop_frames_bound(num_frames), the
+ * largest byte_offset[f + k - 1] + byte_len[f + k - 1] - byte_offset[f] over every frame f, k = min(S, frames of f's
+ * file from f on).  Host only, O(n_frames).  0 for num_frames 0 or a bad file_frames. */
+size_t clx_crop_bytes_bound(const clx_frame_desc* descs, size_t n_frames, const uint32_t* file_frames, size_t n_files,
+                            size_t num_frames);
 /* A crop batch of n_crops excerpts of num_frames samples each, in mode CLX_OUT_CHANNELS_I32 or _F32.  It is an ordinary
  * clx_batch (clx_batch_decode, _sync, _last_kernel_ms, _read_to, clx_ctx_run_steps, clx_batch_device_out work on it)
  * that shares the corpus's bytes.  Output: [n_crops * C, num_frames] channels-first, C the corpus's largest channel
@@ -303,7 +321,10 @@ size_t clx_crop_frames_bound(const clx_frame_desc* descs, size_t n_frames, const
  * unspecified.  The frame CRC-16 is checked on the device in every decode (frames the demuxer confirmed are skipped).
  * F32 is refused when ANY frame of the corpus has more than 24 bits, since the batch may be asked for any of them.
  * Memory: (n_crops + 1) * C * num_frames output elements (the C rows after the output take the unused slots) and, per
- * slot, a planar scratch of the corpus's largest frame; slots = n_crops * clx_crop_frames_bound(num_frames).
+ * slot, a planar scratch of the corpus's largest frame; slots = n_crops * clx_crop_frames_bound(num_frames).  Over a
+ * host corpus (CLX_CORPUS_HOST), also a staging buffer of n_crops spans of clx_crop_bytes_bound(num_frames) + 15 bytes
+ * rounded up to 16, plus the filler frame and 128 to 191 bytes of slack; each decode reads every selected crop's span
+ * (at most that bound per crop) from host memory over PCIe.
  * CLX_ERR_INVALID_ARGUMENT for: n_crops or num_frames 0, n_crops of 2^30 or more, slots of 2^32 or more, sizes that
  * overflow, a mode other than the two channels modes, F32 with a frame above 24 bits. */
 typedef struct clx_crop_request {

@@ -7,11 +7,16 @@ bench_crops.py's workload: C2-shaped files (16-bit stereo, 4096-sample frames), 
    per call from CUDA events on torch's stream around `--calls` calls (the request copies, the graph, the waits);
 2. the same calls with check=True (one sync each), host clock per call;
 3. load_crops() calls, host clock per call;
-4. bench_crops.py's part 1: resident windowed batches of the same shape, Context.run_steps over `--streams` streams.
+4. bench_crops.py's part 1: resident windowed batches of the same shape, Context.run_steps over `--streams` streams;
+5. part 1 over a host corpus (Corpus(memory="host")) of the same files, the same draws: each call also gathers the
+   crops' spans of frames from pinned host memory over PCIe.
 
-Every crop-batch draw of part 1 is checked bit for bit against load_crops() of the same requests once, before the
-timed rounds.  The card's name, power limit and SM clock are read in the same run; memory of the crop batch is
-reported (corpus bytes, planar scratch, output).  One JSON line.
+Every crop-batch draw of parts 1 and 5 is checked bit for bit against load_crops() of the same requests once (and the
+two batches against each other), before the timed rounds.  A separate torch.profiler run of `--profile-calls` host-corpus
+calls gives the gather kernel's own time and the planner kernels'; the bytes each call gathers are computed on the host
+from the plan (plan_range over every crop of every draw), and over the gather's time give its PCIe rate.  The card's
+name, power limit and SM clock are read in the same run; memory of the crop batches is reported (corpus bytes and the
+device memory of each corpus, planar scratch, output, the host-corpus batch's staging buffer).  One JSON line.
 
     python tools/bench_corpus.py
     python tools/bench_corpus.py --rounds 3 --calls 100
@@ -39,6 +44,36 @@ def stats(v):
             "spread": round((float(np.max(v)) - float(np.min(v))) / med, 4) if med else 0.0}
 
 
+def gathered_bytes(corpus, fi, off, n):
+    """Bytes the gather copies for one call: per crop, from its first planned frame's start to its last one's end."""
+    total = 0
+    for f, o in zip(fi.tolist(), off.tolist()):
+        x = corpus.index[f]
+        sel, _, _ = cb.plan_range(x.descs, o, min(o + n, x.length), starts=x.starts)
+        if sel.size:
+            total += int(x.descs["byte_offset"][sel[-1]]) + int(x.descs["byte_len"][sel[-1]]) - int(x.descs["byte_offset"][sel[0]])
+    return total
+
+
+def profile_kernels(batch, draws):
+    """Device time per call of each crop_* kernel (us), from a torch.profiler run of its own."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for fi, off in draws:
+            batch(fi, off, check=False)
+        torch.cuda.synchronize()
+    us = {}
+    for e in prof.key_averages():
+        t = getattr(e, "device_time_total", None)
+        t = getattr(e, "cuda_time_total", 0) if t is None else t
+        if t and "crop_" in e.key:
+            name = e.key.split("(")[0].split("::")[-1].split("<")[0].strip()
+            us[name] = round(us.get(name, 0.0) + t / len(draws), 2)
+    return us
+
+
 def main():
     import torch
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
@@ -52,6 +87,7 @@ def main():
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--streams", type=int, default=4)
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--profile-calls", type=int, default=20, help="host-corpus calls in the torch.profiler run")
     ap.add_argument("--out", default=None, help="also append the JSON line to this file")
     args = ap.parse_args()
     n, B = args.num_frames, args.batch
@@ -63,8 +99,13 @@ def main():
     batch = corpus.crops(B, n, dtype=torch.float32)
     slots = B * corpus.frames_bound(n)
     slot_elems = (max(192, int((corpus.descs["n_channels"].astype(np.int64) * corpus.descs["block_size"]).max())) + 3) & ~3
+    host = cb.Corpus(idx, ctx, memory="host")
+    hbatch = host.crops(B, n, dtype=torch.float32)
+    span_stride = (host.bytes_bound(n) + 30) & ~15
     memory = {"corpus_bytes": corpus.nbytes, "slots": slots, "planar_scratch_bytes": slots * slot_elems * 4,
-              "output_bytes": B * corpus.channels * n * 4, "trash_rows_bytes": corpus.channels * n * 4}
+              "output_bytes": B * corpus.channels * n * 4, "trash_rows_bytes": corpus.channels * n * 4,
+              "device_corpus_device_bytes": corpus.device_bytes, "host_corpus_device_bytes": host.device_bytes,
+              "host_batch_staging_bytes": B * span_stride, "crop_bytes_bound": host.bytes_bound(n)}
 
     # requests drawn on the device; the largest offset keeps every crop whole, as in bench_crops.py
     lens = torch.tensor([f.length for f in idx.files], device="cuda")
@@ -74,11 +115,17 @@ def main():
         fi = torch.randint(0, len(idx), (B,), device="cuda", generator=gen)
         off = (torch.rand(B, device="cuda", generator=gen) * (lens[fi] - n + 1).double()).long()
         draws.append((fi, off))
-    exact = True
+    exact, host_exact = True, True
     for fi, off in draws[:3]:
         out, lengths = batch(fi, off)
         exp, elen = cb.load_crops(idx, fi.tolist(), off.tolist(), n, ctx=ctx)
         exact &= bool(torch.equal(out.view(torch.int32), exp.view(torch.int32)) and torch.equal(lengths.cpu(), elen))
+        out_d = out.clone()
+        out, lengths = hbatch(fi, off)
+        host_exact &= bool(torch.equal(out.view(torch.int32), exp.view(torch.int32)) and torch.equal(lengths.cpu(), elen)
+                           and torch.equal(out.view(torch.int32), out_d.view(torch.int32)))
+    per_call = [gathered_bytes(host, fi, off, n) for fi, off in draws]
+    gathered = {"mean_per_call": int(np.mean(per_call)), "min": int(np.min(per_call)), "max": int(np.max(per_call))}
 
     win = []
     for _ in range(args.units):
@@ -88,18 +135,24 @@ def main():
     ctx.run_steps(win, args.units * 2, args.streams)
     for fi, off in draws[:5]:
         batch(fi, off, check=False)
+        hbatch(fi, off, check=False)
     torch.cuda.synchronize()
 
-    ms = {"crop_batch_device": [], "crop_batch_checked_host": [], "load_crops_host": [], "windowed_resident_device": []}
-    for _ in range(args.rounds):
+    def device_ms(b):  # device time per call, back to back over every draw
         start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         torch.cuda.synchronize()
         start.record()
         for fi, off in draws:
-            batch(fi, off, check=False)
+            b(fi, off, check=False)
         stop.record()
         stop.synchronize()
-        ms["crop_batch_device"].append(start.elapsed_time(stop) / len(draws))
+        return start.elapsed_time(stop) / len(draws)
+
+    ms = {"crop_batch_device": [], "host_corpus_crop_batch_device": [], "crop_batch_checked_host": [],
+          "load_crops_host": [], "windowed_resident_device": []}
+    for _ in range(args.rounds):
+        ms["crop_batch_device"].append(device_ms(batch))
+        ms["host_corpus_crop_batch_device"].append(device_ms(hbatch))
         per = []
         for fi, off in draws:
             t0 = time.perf_counter()
@@ -119,17 +172,24 @@ def main():
     info = gpu_info()
     for dev in win:
         dev.close()
+    kernels_us = profile_kernels(hbatch, draws[:args.profile_calls])
+    prof_bytes = float(np.mean(per_call[:args.profile_calls]))
+    gather_us = kernels_us.get("crop_gather_kernel")
+    host_ms = float(np.median(ms["host_corpus_crop_batch_device"]))
+    gathered.update({"gather_kernel_GBps": round(prof_bytes / (gather_us * 1e3), 2) if gather_us else None,
+                     "over_whole_call_GBps": round(gathered["mean_per_call"] / (host_ms * 1e6), 2)})
     row = {"bench": "corpus_crops", "batch": B, "num_frames": n, "files": args.files, "frames_per_file": args.frames,
            "rounds": args.rounds, "calls": args.calls, "bit_exact_vs_load_crops": exact,
+           "host_corpus_bit_exact_vs_load_crops_and_device_corpus": host_exact,
            "ms_per_call": {k: stats(v) for k, v in ms.items()}, "ms_rounds": {k: [round(x, 4) for x in v] for k, v in ms.items()},
-           "memory": memory, "gpu": info}
+           "host_corpus_kernels_us_per_call": kernels_us, "gathered_bytes": gathered, "memory": memory, "gpu": info}
     line = json.dumps(row)
     print(line, flush=True)
     if args.out:
         with open(args.out, "a") as f:
             f.write(line + "\n")
-    del batch
-    corpus = None
+    del batch, hbatch
+    corpus = host = None
     ctx.close()
 
 

@@ -306,6 +306,48 @@ def _out_array(out_elems: int, mode: int) -> np.ndarray:
 _CHANNEL_MODES = (OUT_CHANNELS_I32, OUT_CHANNELS_F32)
 
 
+class _Batch:
+    """Owns a clx_batch: the one place that decodes, times and destroys one.  `keep`: what must outlive the batch (a
+    crop batch's corpus).  The tensors that view the batch's buffers hold this handle, not the DeviceBatch or CropBatch
+    around it, so the batch lives as long as the last of them."""
+
+    def __init__(self, ctx: Context, h, keep=None):
+        self.ctx, self.h, self.keep = ctx, h, keep
+
+    def decode(self, stream: int):
+        _check(self.ctx._L.clx_batch_decode(self.ctx._h, self.h, stream), self.ctx)
+
+    def kernel_ms(self) -> float:
+        ms = C.c_float(0)
+        _check(self.ctx._L.clx_batch_last_kernel_ms(self.ctx._h, self.h, C.byref(ms)), self.ctx)
+        return float(ms.value)
+
+    def tensor(self, ptr: int, shape: tuple, typestr: str):
+        """A zero-copy torch CUDA tensor over device memory of the batch; it keeps the batch alive."""
+        import torch
+        return torch.as_tensor(_DeviceView(self, ptr, shape, typestr), device="cuda")
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.ctx, "_h", None):
+            self.ctx._L.clx_batch_destroy(self.ctx._h, self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class _DeviceView:
+    """__cuda_array_interface__ of device memory owned by `owner`, which it keeps alive while a tensor views it."""
+
+    def __init__(self, owner, ptr: int, shape: tuple, typestr: str):
+        self.owner = owner
+        self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (int(ptr), False), "strides": None,
+                                         "version": 2}
+
+
 class DeviceBatch:
     """clx_batch: frames resident in HBM; decode() launches the kernels only."""
 
@@ -353,19 +395,21 @@ class DeviceBatch:
         else:
             _check(ctx._L.clx_batch_create_to(ctx._h, ptr, self.nbytes, self.descs.ctypes.data, self.descs.size,
                                               self.out_elems, flags, self.mode, C.byref(h)), ctx)
-        self._h = h
+        self._batch = _Batch(ctx, h)
+
+    @property
+    def _h(self):
+        return self._batch.h
 
     def decode(self, stream: int = 0):
-        _check(self.ctx._L.clx_batch_decode(self.ctx._h, self._h, stream), self.ctx)
+        self._batch.decode(stream)
         self._stream = stream
 
     def sync(self):
         _check(self.ctx._L.clx_batch_sync(self.ctx._h, self._h), self.ctx)
 
     def kernel_ms(self) -> float:
-        ms = C.c_float(0)
-        _check(self.ctx._L.clx_batch_last_kernel_ms(self.ctx._h, self._h, C.byref(ms)), self.ctx)
-        return float(ms.value)
+        return self._batch.kernel_ms()
 
     def read(self):
         """Returns (out, results); `out` is in the batch's mode: int32, int16, or uint8 with 3 bytes per sample; in a
@@ -397,33 +441,15 @@ class DeviceBatch:
         if self._stream is not None:
             ptr = self.ctx._L.clx_ctx_stream(self.ctx._h, self._stream)
             torch.cuda.current_stream().wait_stream(torch.cuda.ExternalStream(ptr))
-        return torch.as_tensor(_CudaArray(self), device="cuda")
+        return self._batch.tensor(self.device_out_ptr, (self.channels, self.channel_stride),
+                                  "<f4" if self.mode == OUT_CHANNELS_F32 else "<i4")
 
     @property
     def device_out_ptr(self) -> int:
         return int(self.ctx._L.clx_batch_device_out(self._h) or 0)
 
     def close(self):
-        if getattr(self, "_h", None) and getattr(self.ctx, "_h", None):
-            self.ctx._L.clx_batch_destroy(self.ctx._h, self._h)
-        self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class _CudaArray:
-    """__cuda_array_interface__ of a channel-mode batch's output; holds the batch while a tensor views it."""
-
-    def __init__(self, batch: DeviceBatch):
-        self.batch = batch
-        self.__cuda_array_interface__ = {
-            "shape": (batch.channels, batch.channel_stride),
-            "typestr": "<f4" if batch.mode == OUT_CHANNELS_F32 else "<i4",
-            "data": (batch.device_out_ptr, False), "strides": None, "version": 2}
+        self._batch.close()
 
 
 _default_ctx: Context | None = None
@@ -804,6 +830,11 @@ def _torch_dtype(dtype):
     return dtype
 
 
+def _channels_mode(dtype) -> int:  # of a dtype _torch_dtype() accepted
+    import torch
+    return OUT_CHANNELS_F32 if dtype == torch.float32 else OUT_CHANNELS_I32
+
+
 def _decode_excerpts(idx: FlacIndex, excerpts, rows: int, stride: int, out, ctx: Context | None, where):
     """Decodes excerpts of indexed files in one windowed batch into `out`, a torch tensor viewing [rows, stride].
     `excerpts`: (file, lo, hi, column, row) per excerpt: samples [lo, hi) of the file go to row `row` + c from
@@ -831,8 +862,8 @@ def _decode_excerpts(idx: FlacIndex, excerpts, rows: int, stride: int, out, ctx:
         return
     descs, windows, owner = np.concatenate(parts), np.concatenate(wins), np.concatenate(owner)
     ctx = ctx or default_context()
-    mode = OUT_CHANNELS_F32 if out.dtype == torch.float32 else OUT_CHANNELS_I32
-    dev = ctx.upload(np.concatenate(chunks), descs, mode=mode, channels=rows, channel_stride=stride, windows=windows)
+    dev = ctx.upload(np.concatenate(chunks), descs, mode=_channels_mode(out.dtype), channels=rows, channel_stride=stride,
+                     windows=windows)
     try:
         dev.decode(0)
         res = dev.results()
@@ -929,15 +960,6 @@ def load_crops(index: FlacIndex, files, offsets, num_frames: int, dtype=None, ct
 # device-resident corpora: crops planned on the device
 # ---------------------------------------------------------------------------
 
-class _DeviceView:
-    """__cuda_array_interface__ of device memory owned by `owner`, which it keeps alive while a tensor views it."""
-
-    def __init__(self, owner, ptr: int, shape: tuple, typestr: str):
-        self.owner = owner
-        self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (int(ptr), False), "strides": None,
-                                         "version": 2}
-
-
 class Corpus:
     """The compressed frames of a FlacIndex's files, copied once with their frame index (clx_corpus_create_ex), for
     CropBatch: crops whose frames, windows and columns are planned on the device.  Each file's bytes from its first
@@ -1013,24 +1035,6 @@ class Corpus:
             pass
 
 
-class _CropHandle:
-    """Owns a crop batch's clx_batch; the tensors that view its buffers keep it (and its corpus) alive."""
-
-    def __init__(self, corpus: Corpus, h):
-        self.corpus, self.ctx, self.h = corpus, corpus.ctx, h
-
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.ctx, "_h", None):
-            self.ctx._L.clx_batch_destroy(self.ctx._h, self.h)
-        self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
 class CropBatch:
     """`batch` excerpts of `num_frames` samples of a Corpus's files per call, as one [B, C, L] CUDA tensor
     (clx_batch_create_crops): the crops' frames, windows and columns are planned on the device inside the batch's CUDA
@@ -1055,16 +1059,13 @@ class CropBatch:
         self.batch, self.num_frames, self.dtype = int(batch), int(num_frames), dtype
         if self.batch < 1 or self.num_frames < 1:
             raise ValueError("batch and num_frames must be >= 1")
-        mode = OUT_CHANNELS_F32 if dtype == torch.float32 else OUT_CHANNELS_I32
+        mode = _channels_mode(dtype)
         L = self.ctx._L
         h = C.c_void_p()
         _check(L.clx_batch_create_crops(self.ctx._h, corpus._h, self.batch, self.num_frames, mode, C.byref(h)), self.ctx)
-        self._handle = _CropHandle(corpus, h)
+        self._batch = _Batch(self.ctx, h, keep=corpus)
         self.channels = corpus.channels
-        B, hd = self.batch, self._handle
-
-        def view(ptr, shape, typestr):
-            return torch.as_tensor(_DeviceView(hd, ptr, shape, typestr), device="cuda")
+        B, view = self.batch, self._batch.tensor
         self.out = view(L.clx_batch_device_out(h), (B, self.channels, self.num_frames),
                         "<f4" if mode == OUT_CHANNELS_F32 else "<i4")
         self.lengths = view(L.clx_batch_crop_lengths(h), (B,), "<i8")
@@ -1101,7 +1102,7 @@ class CropBatch:
         self._requests[:, 0].copy_(files)
         self._requests[:, 1].copy_(offsets)
         self._stream.wait_stream(torch.cuda.current_stream())
-        _check(self.ctx._L.clx_batch_decode(self.ctx._h, self._handle.h, 0), self.ctx)
+        self._batch.decode(0)
         torch.cuda.current_stream().wait_stream(self._stream)
         if check:
             self._raise()
@@ -1122,6 +1123,4 @@ class CropBatch:
 
     def kernel_ms(self) -> float:
         """Device time of the last call's graph (CUDA events), planner and status pass included."""
-        ms = C.c_float(0)
-        _check(self.ctx._L.clx_batch_last_kernel_ms(self.ctx._h, self._handle.h, C.byref(ms)), self.ctx)
-        return float(ms.value)
+        return self._batch.kernel_ms()

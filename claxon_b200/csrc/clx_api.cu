@@ -22,8 +22,8 @@
 #include "claxon_b200.h"
 #include "clx_internal.h"
 
-// A few long-lived host threads for the per-call CRC-16 pass: spawning std::threads per call costs more
-// than the checksums themselves (6 MB per C2 batch).
+// A few long-lived host threads for the frame CRC-16 pass of batch creation from host bytes (precompute_crc):
+// spawning std::threads per batch costs more than the checksums themselves (6 MB per C2 batch).
 class HostPool {
 public:
     explicit HostPool(unsigned n) {
@@ -88,39 +88,113 @@ private:
     bool stop_ = false;
 };
 
+namespace {
+// The size of a device buffer for `nbytes` frame bytes: whole 64-byte TMA chunks + 128 bytes of look-ahead
+// (clx::DecodeBuffers' contract).
+size_t padded_bytes(size_t nbytes) { return ((nbytes + 63) & ~(size_t)63) + 128; }
+
+bool is_channels(uint32_t mode) { return mode == CLX_OUT_CHANNELS_I32 || mode == CLX_OUT_CHANNELS_F32; }
+
+// What one decode needs: `nbytes` frame bytes (before padding), `n_frames` frames, `planar` elements of planar i32
+// output or scratch, and unless in CLX_OUT_PLANAR_I32, `conv` elements of output in `mode` and with `mark` a mark byte
+// per frame (device-resident batches: their lane-per-frame decode writes `conv` itself).
+struct DecodeNeed {
+    size_t nbytes, n_frames, planar;
+    uint32_t mode;
+    size_t conv;
+    bool mark;
+    clx::Plan plan;
+};
+
+// Owns the device buffers of one decode, which clx::DecodeBuffers views, and is the only code that knows their sizes.
+// A batch sizes them once, exactly; the host-buffer call keeps one set per stream and only ever grows it.  Borrowed
+// frame bytes (a crop batch's over a device corpus) are neither allocated nor freed here.
+struct DecodeStorage {
+    uint8_t* bytes = nullptr; size_t buf_bytes = 0, bytes_cap = 0;
+    bool borrowed = false;
+    clx_frame_desc* descs = nullptr; size_t descs_cap = 0;
+    int32_t* out = nullptr; size_t out_cap = 0;
+    clx_frame_result* results = nullptr; size_t results_cap = 0;
+    int* flags = nullptr;
+    uint8_t* params = nullptr; size_t params_cap = 0;
+    uint8_t* conv = nullptr; size_t conv_cap = 0;
+    uint8_t* mark = nullptr; size_t mark_cap = 0;
+    uint64_t* cols = nullptr; size_t cols_cap = 0;
+    uint32_t* wins = nullptr; size_t wins_cap = 0;
+
+    void borrow(uint8_t* p, size_t padded) { bytes = p; buf_bytes = padded; borrowed = true; }
+
+    // Makes every buffer `n` asks for large enough.  !grow (a batch): exactly as large, zeroing the frame bytes, and in
+    // a channels mode the output (elements no window covers read 0).  grow (the host-buffer call): a buffer that is too
+    // small is reallocated with headroom, and nothing is zeroed.
+    cudaError_t fit(const DecodeNeed& n, bool grow) {
+        const bool channels = is_channels(n.mode);
+        const size_t frames = std::max<size_t>(1, n.n_frames);
+        const size_t conv_bytes = (n.conv + 8) * clx::output_elem_size(n.mode);
+        cudaError_t e = cudaSuccess;
+        if (!borrowed) {
+            buf_bytes = padded_bytes(n.nbytes);
+            e = fit_one(bytes, bytes_cap, buf_bytes, 4096, grow);
+            if (e == cudaSuccess && !grow) e = cudaMemset(bytes, 0, buf_bytes);
+        }
+        if (e == cudaSuccess) e = fit_one(descs, descs_cap, frames, 64, grow);
+        if (e == cudaSuccess) e = fit_one(out, out_cap, n.planar + 4, 4096, grow);
+        if (e == cudaSuccess) e = fit_one(results, results_cap, frames, 64, grow);
+        if (e == cudaSuccess && !flags) e = cudaMalloc((void**)&flags, 4 * sizeof(int));
+        if (e == cudaSuccess) e = fit_one(params, params_cap, clx::coop_params_bytes(n.plan, (uint32_t)n.n_frames) + 16, 4096, grow);
+        if (e == cudaSuccess && n.mode != CLX_OUT_PLANAR_I32) e = fit_one(conv, conv_cap, conv_bytes, 4096, grow);
+        if (e == cudaSuccess && channels && !grow) e = cudaMemset(conv, 0, conv_bytes);
+        if (e == cudaSuccess && n.mark && n.mode != CLX_OUT_PLANAR_I32) e = fit_one(mark, mark_cap, frames, 0, grow);
+        if (e == cudaSuccess && channels) e = fit_one(cols, cols_cap, frames, 0, grow);
+        if (e == cudaSuccess && channels) e = fit_one(wins, wins_cap, frames, 0, grow);
+        return e;
+    }
+
+    clx::DecodeBuffers view(uint32_t n_frames, uint32_t mode, uint64_t stride) const {
+        return clx::DecodeBuffers{bytes, buf_bytes, descs, n_frames, out, results, flags, params, mode, conv, mark, cols,
+                                  stride, wins};
+    }
+
+    void release() {
+        if (!borrowed) cudaFree(bytes);
+        cudaFree(descs); cudaFree(out); cudaFree(results); cudaFree(flags); cudaFree(params);
+        cudaFree(conv); cudaFree(mark); cudaFree(cols); cudaFree(wins);
+    }
+
+private:
+    // `p` holds at least `need` elements afterwards: when it had to be reallocated, exactly that many, or with `grow`
+    // a quarter more plus `slack`.
+    template <typename T>
+    static cudaError_t fit_one(T*& p, size_t& cap, size_t need, size_t slack, bool grow) {
+        if (p && need <= cap) return cudaSuccess;
+        cudaError_t e = cudaFree(p);
+        p = nullptr; cap = 0;
+        const size_t want = grow ? need + need / 4 + slack : need;
+        if (e == cudaSuccess) e = cudaMalloc((void**)&p, want * sizeof(T));
+        if (e == cudaSuccess) cap = want;
+        return e;
+    }
+};
+}  // namespace
+
 struct clx_ctx {
     int device = 0;
     uint32_t flags = 0;
     std::vector<cudaStream_t> streams;
     std::string last_error;
     uint64_t launches = 0;
-    // grow-only device scratch for clx_decode_frames, one set per stream (chunk pipelining)
-    struct Scratch {
-        uint8_t* d_bytes = nullptr; size_t bytes_cap = 0;
-        clx_frame_desc* d_descs = nullptr; size_t descs_cap = 0;
-        int32_t* d_out = nullptr; size_t out_cap = 0;
-        clx_frame_result* d_results = nullptr; size_t results_cap = 0;
-        int* d_need_hi = nullptr;
-        uint8_t* d_params = nullptr; size_t params_cap = 0;  // fast path: per-subframe predictor parameters
-        uint8_t* d_conv = nullptr; size_t conv_cap = 0;      // interleaved output modes: converted samples
-    };
-    std::vector<Scratch> scratch;
+    std::vector<DecodeStorage> scratch;  // clx_decode_frames: one grow-only set per stream (chunk pipelining)
     // pinned staging for the small per-frame tables: pageable memory would make the "async" copies
     // synchronous and serialise the chunk pipeline
     clx_frame_desc* h_descs = nullptr; size_t h_descs_cap = 0;   // rebased descriptors (H2D)
     clx_frame_result* h_results = nullptr; size_t h_results_cap = 0;  // results (D2H)
-    std::vector<uint8_t> crc_verdict;     // per frame: CRC-16 of the claimed span matched
     unsigned host_threads = 1;
     HostPool* pool = nullptr;   // created on first use
 };
 
 struct clx_batch {
-    uint8_t* d_bytes = nullptr; size_t nbytes = 0, buf_bytes = 0;
-    clx_frame_desc* d_descs = nullptr;
-    int32_t* d_out = nullptr; size_t out_elems = 0;
-    clx_frame_result* d_results = nullptr;
-    int* d_need_hi = nullptr;
-    void* d_params = nullptr;
+    DecodeStorage buf;
+    size_t out_elems = 0;
     uint32_t n_frames = 0;
     cudaEvent_t ev_start = nullptr, ev_stop = nullptr;
     cudaStream_t last_stream = nullptr;
@@ -137,22 +211,18 @@ struct clx_batch {
     std::vector<uint32_t> h_len;
     std::vector<uint32_t> order;   // device position -> caller's frame index (empty: identity), see shape_order()
     bool device_crc = false;       // bytes came from device memory: the CRC-16 check runs on the device, inside the graph
-    // Output mode (CLX_OUT_*).  Interleaved batches hand out d_conv; d_out stays their planar scratch.  The lane-per-frame
-    // path writes I32 / I16 into d_conv itself (d_mark: the frames the generic kernel took over); every other path, and
-    // I24, decodes to d_out and converts all frames inside the graph (see clx::launch_decode).
-    // Channels modes: d_conv holds out_elems = rows * stride elements, and the device descriptors' out_offset is the
-    // frame's place in the planar scratch d_out (frames packed back to back, 4-element aligned); d_cols holds each
-    // frame's window start on row 0 (row base * stride + column), and d_wins its window (first | count << 16; full windows
-    // for clx_batch_create_channels), both in the device order.
+    // Output mode (CLX_OUT_*).  Interleaved batches hand out buf.conv; buf.out stays their planar scratch.  The
+    // lane-per-frame path writes I32 / I16 into buf.conv itself (buf.mark: the frames the generic kernel took over); every
+    // other path, and I24, decodes to buf.out and converts all frames inside the graph (see clx::launch_decode).
+    // Channels modes: buf.conv holds out_elems = rows * stride elements, and the device descriptors' out_offset is the
+    // frame's place in the planar scratch buf.out (frames packed back to back, 4-element aligned); buf.cols holds each
+    // frame's window start on row 0 (row base * stride + column), and buf.wins its window (first | count << 16; full
+    // windows for clx_batch_create_channels), both in the device order.
     uint32_t mode = CLX_OUT_PLANAR_I32;
-    void* d_conv = nullptr;
-    uint8_t* d_mark = nullptr;
-    uint64_t* d_cols = nullptr;
-    uint32_t* d_wins = nullptr;
     uint64_t stride = 0;
-    // Crop batches (clx_batch_create_crops): d_bytes is the corpus's, not the batch's; the planner writes d_descs,
-    // d_cols and d_wins in every decode (clx_crops.cu).  Over a host corpus, d_bytes is the batch's own staging buffer:
-    // n_crops spans of span_stride bytes, then the filler frame.
+    // Crop batches (clx_batch_create_crops): buf.bytes is the corpus's, not the batch's; the planner writes buf.descs,
+    // buf.cols and buf.wins in every decode (clx_crops.cu).  Over a host corpus, buf.bytes is the batch's own staging
+    // buffer: n_crops spans of span_stride bytes, then the filler frame.
     clx_corpus* corpus = nullptr;
     clx::CropBuffers crop{};
     uint64_t span_stride = 0;
@@ -192,18 +262,6 @@ int cuda_fail(clx_ctx* ctx, cudaError_t e, const char* what) {
         if (e_ != cudaSuccess) return cuda_fail(ctx, e_, #call);   \
     } while (0)
 
-template <typename T>
-int grow(clx_ctx* ctx, T*& ptr, size_t& cap, size_t need, size_t slack) {
-    if (need <= cap && ptr) return CLX_OK;
-    if (ptr) CU(ctx, cudaFree(ptr));
-    ptr = nullptr;
-    cap = 0;
-    size_t want = need + need / 4 + slack;
-    CU(ctx, cudaMalloc((void**)&ptr, want * sizeof(T)));
-    cap = want;
-    return CLX_OK;
-}
-
 // Host-side frame CRC-16 (src/frame.rs:752-763) for device-resident batches: their bytes never change, so the
 // checksum of every claimed span is taken once, when the batch is created (the host-buffer call checks on the
 // device instead, clx_crc.cu).  It takes effect only when the subframes decoded, so subframe errors keep their
@@ -219,10 +277,9 @@ void precompute_crc_range(const uint8_t* bytes, const clx_frame_desc* descs, uin
     }
 }
 
-void precompute_crc(clx_ctx* ctx, const uint8_t* bytes, const clx_frame_desc* descs, size_t n) {
-    ctx->crc_verdict.assign(n, 0);
-    if (ctx->flags & CLX_OPT_NO_VERIFY_CRC) return;
-    uint8_t* verdict = ctx->crc_verdict.data();
+void precompute_crc(clx_ctx* ctx, const uint8_t* bytes, const clx_frame_desc* descs, size_t n, std::vector<uint8_t>& out) {
+    out.assign(n, 0);
+    uint8_t* verdict = out.data();
     unsigned nt = std::min<unsigned>(ctx->host_threads, (unsigned)std::max<size_t>(1, n / 32));
     if (nt <= 1) return precompute_crc_range(bytes, descs, verdict, 0, n);
     if (!ctx->pool) ctx->pool = new HostPool(ctx->host_threads - 1);
@@ -232,28 +289,61 @@ void precompute_crc(clx_ctx* ctx, const uint8_t* bytes, const clx_frame_desc* de
 }
 
 void build_graph(clx_ctx* ctx, clx_batch* b);
-int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
-                 const clx_frame_window* windows, size_t n_frames, size_t out_elems, uint32_t batch_flags, uint32_t mode,
-                 bool channels, uint32_t n_rows, size_t stride, clx_batch** out);
 
-// The interleaved modes hold a sample in 2 / 3 bytes only for frames of at most 16 / 24 bits per sample.
-bool frames_fit_mode(const clx_frame_desc* descs, size_t n_frames, uint32_t mode) {
-    const uint32_t max_bps = mode == CLX_OUT_INTERLEAVED_I16 ? 16u : mode == CLX_OUT_INTERLEAVED_I24 ? 24u : 32u;
-    for (size_t i = 0; i < n_frames; i++)
-        if (descs[i].bits_per_sample > max_bps) return false;
+// Where a create or decode call writes its `out_elems` samples.  Planar and interleaved modes: each frame from its
+// out_offset on.  Channels modes: `n_rows` rows of `stride` elements; frame i stores its window windows[i] (null: every
+// frame its full window at row 0) from column out_offset on.
+struct Output {
+    uint32_t mode;
+    size_t out_elems;
+    uint32_t n_rows;
+    size_t stride;
+    const clx_frame_window* windows;
+};
+
+// Everything the kernels assume about a call's frames (the C ABI trusts none of it): the bytes and descriptors are
+// given, and each frame lies in the bytes and has a shape the kernels decode.  With `o`, each frame also fits the
+// output: the mode's sample width (interleaved I16: 16 bits, I24 and channels F32: 24), and its range of out_elems, or
+// in a channels mode its window, rows and columns.  Without (a corpus), the bytes alone.
+bool valid_frames(const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames, const Output* o) {
+    if ((!bytes && nbytes) || (!descs && n_frames)) return false;
+    const bool channels = o && is_channels(o->mode);
+    if (channels && (o->n_rows == 0 || o->stride == 0 || o->stride > SIZE_MAX / 4 / o->n_rows)) return false;
+    const uint32_t max_bps = !o ? 32u : o->mode == CLX_OUT_INTERLEAVED_I16 ? 16u :
+                             o->mode == CLX_OUT_INTERLEAVED_I24 || o->mode == CLX_OUT_CHANNELS_F32 ? 24u : 32u;
+    for (size_t i = 0; i < n_frames; i++) {
+        const clx_frame_desc& d = descs[i];
+        const uint32_t bps = d.bits_per_sample;
+        if (!(d.byte_offset <= nbytes && d.byte_len <= nbytes - d.byte_offset && d.header_len <= d.byte_len &&
+              d.n_channels >= 1 && d.n_channels <= 8 && d.block_size != 0 && d.byte_len <= (1u << 28) &&
+              !(d.channel_assignment >= 8 && d.n_channels != 2) && d.channel_assignment <= 10 &&
+              (bps == 0 || (bps >= 4 && bps <= max_bps))))  // 0: "not in the header" -> Unsupported, as the reference
+            return false;
+        if (!o) continue;
+        const uint64_t elems = (uint64_t)d.n_channels * d.block_size;
+        if (!channels) {
+            if (d.out_offset > o->out_elems || elems > o->out_elems - d.out_offset) return false;
+            continue;
+        }
+        const clx_frame_window w = o->windows ? o->windows[i] : clx_frame_window{0, 0, d.block_size, 0};
+        if (!(w.reserved == 0 && w.row <= o->n_rows && d.n_channels <= o->n_rows - w.row && w.first < d.block_size &&
+              w.count != 0 && w.count <= (uint32_t)d.block_size - w.first && d.out_offset <= o->stride &&
+              w.count <= o->stride - d.out_offset))
+            return false;
+    }
     return true;
 }
 
-// Everything the kernels assume about a caller-supplied descriptor (the C ABI does not trust it).
-bool valid_desc(const clx_frame_desc& d, size_t nbytes, size_t out_elems) {
-    const uint64_t elems = (uint64_t)d.n_channels * d.block_size;
-    const uint32_t bps = d.bits_per_sample;
-    return d.byte_offset <= nbytes && d.byte_len <= nbytes - d.byte_offset && d.header_len <= d.byte_len &&
-           d.n_channels >= 1 && d.n_channels <= 8 && d.block_size != 0 && d.byte_len <= (1u << 28) &&
-           !(d.channel_assignment >= 8 && d.n_channels != 2) && d.channel_assignment <= 10 &&
-           (bps == 0 || (bps >= 4 && bps <= 32)) &&  // 0: "not in the header" -> Unsupported, as the reference
-           d.out_offset <= out_elems && elems <= out_elems - d.out_offset;
+// Copies per-frame results from the device order to the caller's frame indices: position p holds frame order[p] (an
+// empty order: the same order).
+void unpermute(const clx_frame_result* dev, const std::vector<uint32_t>& order, size_t n, clx_frame_result* results) {
+    if (order.empty()) memcpy(results, dev, n * sizeof(clx_frame_result));
+    else
+        for (size_t p = 0; p < n; p++) results[order[p]] = dev[p];
 }
+
+int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
+                 uint32_t batch_flags, const Output& o, clx_batch** out);
 
 // The kernels map consecutive descriptors onto the lanes of a warp, and a warp advances at the pace of its longest
 // block: frames of one shape belong next to each other.  Fills `order` (position -> frame index) with the frames
@@ -335,11 +425,7 @@ int clx_ctx_create(const clx_options* opts, clx_ctx** out) {
 void clx_ctx_destroy(clx_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    for (auto& s : ctx->scratch) {
-        cudaFree(s.d_bytes); cudaFree(s.d_descs); cudaFree(s.d_out); cudaFree(s.d_results); cudaFree(s.d_need_hi);
-        cudaFree(s.d_params);
-        cudaFree(s.d_conv);
-    }
+    for (auto& s : ctx->scratch) s.release();
     for (auto s : ctx->streams) cudaStreamDestroy(s);
     if (ctx->h_descs) cudaFreeHost(ctx->h_descs);
     if (ctx->h_results) cudaFreeHost(ctx->h_results);
@@ -361,16 +447,14 @@ int clx_decode_frames(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const c
 
 int clx_decode_frames_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
                          size_t n_frames, void* out_v, size_t out_elems, clx_frame_result* results, uint32_t mode) {
-    if (!ctx || (!bytes && nbytes) || (!descs && n_frames) || (!results && n_frames) || mode > CLX_OUT_INTERLEAVED_I24)
+    const Output o{mode, out_elems, 0, 0, nullptr};
+    if (!ctx || (!results && n_frames) || mode > CLX_OUT_INTERLEAVED_I24 || !valid_frames(bytes, nbytes, descs, n_frames, &o))
         return CLX_ERR_INVALID_ARGUMENT;
     if (n_frames == 0) return CLX_OK;
     uint8_t* const out = static_cast<uint8_t*>(out_v);
     const size_t esize = clx::output_elem_size(mode);
-    if (!frames_fit_mode(descs, n_frames, mode)) return CLX_ERR_INVALID_ARGUMENT;
-    CU(ctx, cudaSetDevice(ctx->device));
     if (!out) return CLX_ERR_INVALID_ARGUMENT;
-    for (size_t i = 0; i < n_frames; i++)
-        if (!valid_desc(descs[i], nbytes, out_elems)) return CLX_ERR_INVALID_ARGUMENT;
+    CU(ctx, cudaSetDevice(ctx->device));
     const double t0 = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
     // Chunks of frames are pipelined over the context's streams: H2D of chunk i+1 and D2H of
     // chunk i-1 overlap the kernels of chunk i.  A chunk covers a contiguous byte range and a
@@ -436,31 +520,21 @@ int clx_decode_frames_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, cons
     } while (0)
     for (size_t c = 0; c < n_chunks; c++) {
         const Span& s = spans[c];
-        clx_ctx::Scratch& sc = ctx->scratch[c];
+        DecodeStorage& sc = ctx->scratch[c];
         cudaStream_t st = ctx->streams[c];
         const size_t nb = (size_t)(s.b1 - s.b0), nf = s.f1 - s.f0, lead = (size_t)(s.o0 & 3), no = (size_t)(s.o1 - s.o0);
-        int rc;
-        const size_t nb_pad = ((nb + 63) & ~(size_t)63) + 128;  // whole 64-byte TMA chunks + look-ahead
-        if ((rc = grow(ctx, sc.d_bytes, sc.bytes_cap, nb_pad, 4096))) return drain(rc);
-        if ((rc = grow(ctx, sc.d_descs, sc.descs_cap, nf, 64))) return drain(rc);
-        if ((rc = grow(ctx, sc.d_out, sc.out_cap, lead + no + 4, 4096))) return drain(rc);
-        if ((rc = grow(ctx, sc.d_results, sc.results_cap, nf, 64))) return drain(rc);
-        if (!sc.d_need_hi) CUD(cudaMalloc((void**)&sc.d_need_hi, 4 * sizeof(int)));
         const clx::Plan plan = make_plan(ctx, descs + s.f0, nf, n_frames <= kLatencyRegimeFrames);
-        if ((rc = grow(ctx, sc.d_params, sc.params_cap, clx::coop_params_bytes(plan, (uint32_t)nf) + 16, 4096))) return drain(rc);
-        if (mode != CLX_OUT_PLANAR_I32 && (rc = grow(ctx, sc.d_conv, sc.conv_cap, (lead + no + 4) * esize, 4096))) return drain(rc);
+        // (never fused: no mark; the frame CRC-16 on the device, src/frame.rs:752-763)
+        CUD(sc.fit({nb, nf, lead + no, mode, lead + no, false, plan}, true));
         enqueued = c + 1;
-        CUD(cudaMemcpyAsync(sc.d_bytes, bytes + s.b0, nb, cudaMemcpyHostToDevice, st));
-        CUD(cudaMemcpyAsync(sc.d_descs, ctx->h_descs + s.f0, nf * sizeof(clx_frame_desc), cudaMemcpyHostToDevice, st));
-        // (never fused: no d_mark; the frame CRC-16 on the device, src/frame.rs:752-763)
-        const clx::DecodeBuffers db{sc.d_bytes, nb_pad, sc.d_descs, (uint32_t)nf, sc.d_out, sc.d_results, sc.d_need_hi,
-                                    sc.d_params, mode, sc.d_conv, nullptr, nullptr, 0, nullptr};
-        CUD(clx::launch_decode(db, plan, !(ctx->flags & CLX_OPT_NO_VERIFY_CRC), st, &ctx->launches));
+        CUD(cudaMemcpyAsync(sc.bytes, bytes + s.b0, nb, cudaMemcpyHostToDevice, st));
+        CUD(cudaMemcpyAsync(sc.descs, ctx->h_descs + s.f0, nf * sizeof(clx_frame_desc), cudaMemcpyHostToDevice, st));
+        CUD(clx::launch_decode(sc.view((uint32_t)nf, mode, 0), plan, !(ctx->flags & CLX_OPT_NO_VERIFY_CRC), st, &ctx->launches));
         if (mode == CLX_OUT_PLANAR_I32)
-            CUD(cudaMemcpyAsync(out + s.o0 * esize, sc.d_out + lead, no * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+            CUD(cudaMemcpyAsync(out + s.o0 * esize, sc.out + lead, no * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         else
-            CUD(cudaMemcpyAsync(out + s.o0 * esize, sc.d_conv + lead * esize, no * esize, cudaMemcpyDeviceToHost, st));
-        CUD(cudaMemcpyAsync(ctx->h_results + s.f0, sc.d_results, nf * sizeof(clx_frame_result), cudaMemcpyDeviceToHost, st));
+            CUD(cudaMemcpyAsync(out + s.o0 * esize, sc.conv + lead * esize, no * esize, cudaMemcpyDeviceToHost, st));
+        CUD(cudaMemcpyAsync(ctx->h_results + s.f0, sc.results, nf * sizeof(clx_frame_result), cudaMemcpyDeviceToHost, st));
     }
 #ifdef CLX_EXPERIMENT
     static const bool trace = getenv("CLX_TRACE") != nullptr;
@@ -472,9 +546,7 @@ int clx_decode_frames_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, cons
     for (size_t c = 0; c < n_chunks; c++) CUD(cudaStreamSynchronize(ctx->streams[c]));
 #undef CUD
     const double t2 = trace ? now() : 0;
-    if (device_order.empty()) memcpy(results, ctx->h_results, n_frames * sizeof(clx_frame_result));
-    else
-        for (size_t p = 0; p < n_frames; p++) results[device_order[p]] = ctx->h_results[p];
+    unpermute(ctx->h_results, device_order, n_frames, results);
     if (trace)
         fprintf(stderr, "[clx] frames=%zu chunks=%zu submit=%.3f ms wait=%.3f ms results=%.3f ms\n", n_frames, n_chunks, t1 - t0,
                 t2 - t1, now() - t2);
@@ -496,14 +568,12 @@ int clx_batch_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const
 
 int clx_batch_create_to(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
                         size_t out_elems, uint32_t batch_flags, uint32_t mode, clx_batch** out) {
-    if (!ctx || !out || (!bytes && nbytes) || (!descs && n_frames) || mode > CLX_OUT_INTERLEAVED_I24)
-        return CLX_ERR_INVALID_ARGUMENT;
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
     *out = nullptr;
-    if (!frames_fit_mode(descs, n_frames, mode)) return CLX_ERR_INVALID_ARGUMENT;
-    CU(ctx, cudaSetDevice(ctx->device));
-    for (size_t i = 0; i < n_frames; i++)
-        if (!valid_desc(descs[i], nbytes, out_elems)) return CLX_ERR_INVALID_ARGUMENT;
-    return create_batch(ctx, bytes, nbytes, descs, nullptr, n_frames, out_elems, batch_flags, mode, false, 0, 0, out);
+    const Output o{mode, out_elems, 0, 0, nullptr};
+    if (!ctx || mode > CLX_OUT_INTERLEAVED_I24 || !valid_frames(bytes, nbytes, descs, n_frames, &o))
+        return CLX_ERR_INVALID_ARGUMENT;
+    return create_batch(ctx, bytes, nbytes, descs, n_frames, batch_flags, o, out);
 }
 
 int clx_batch_create_channels(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
@@ -511,9 +581,10 @@ int clx_batch_create_channels(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes,
                               uint32_t mode, clx_batch** out) {
     if (!out) return CLX_ERR_INVALID_ARGUMENT;
     *out = nullptr;
-    if (n_channels > 8) return CLX_ERR_INVALID_ARGUMENT;
-    return create_batch(ctx, bytes, nbytes, descs, nullptr, n_frames, 0, batch_flags, mode, true, n_channels,
-                        channel_stride, out);
+    const Output o{mode, (size_t)n_channels * channel_stride, n_channels, channel_stride, nullptr};
+    if (!ctx || n_channels > 8 || !is_channels(mode) || !valid_frames(bytes, nbytes, descs, n_frames, &o))
+        return CLX_ERR_INVALID_ARGUMENT;
+    return create_batch(ctx, bytes, nbytes, descs, n_frames, batch_flags, o, out);
 }
 
 int clx_batch_create_windows(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
@@ -521,53 +592,26 @@ int clx_batch_create_windows(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, 
                              uint32_t batch_flags, uint32_t mode, clx_batch** out) {
     if (!out) return CLX_ERR_INVALID_ARGUMENT;
     *out = nullptr;
-    if (!windows && n_frames) return CLX_ERR_INVALID_ARGUMENT;
-    return create_batch(ctx, bytes, nbytes, descs, windows, n_frames, 0, batch_flags, mode, true, n_rows, row_stride, out);
+    const Output o{mode, (size_t)n_rows * row_stride, n_rows, row_stride, windows};
+    if (!ctx || (!windows && n_frames) || !is_channels(mode) || !valid_frames(bytes, nbytes, descs, n_frames, &o))
+        return CLX_ERR_INVALID_ARGUMENT;
+    return create_batch(ctx, bytes, nbytes, descs, n_frames, batch_flags, o, out);
 }
 
 }  // extern "C"
 
 namespace {
-// Everything the channels modes require of a frame and its window (`w`: null for the full window at row 0), beyond
-// the byte-range conditions of valid_desc.
-bool valid_window(const clx_frame_desc& d, const clx_frame_window* w, size_t nbytes, uint32_t n_rows, size_t stride,
-                  uint32_t mode) {
-    const clx_frame_window full{0, 0, d.block_size, 0};
-    if (!w) w = &full;
-    clx_frame_desc at0 = d;  // the byte-range conditions, with the frame alone in its own output
-    at0.out_offset = 0;
-    return valid_desc(at0, nbytes, (size_t)d.n_channels * d.block_size) && w->reserved == 0 &&
-           w->row <= n_rows && d.n_channels <= n_rows - w->row && w->first < d.block_size && w->count != 0 &&
-           w->count <= (uint32_t)d.block_size - w->first && d.out_offset <= stride && w->count <= stride - d.out_offset &&
-           !(mode == CLX_OUT_CHANNELS_F32 && d.bits_per_sample > 24);
-}
-
-// The part of batch creation every mode shares.  !channels: a planar or interleaved mode, whose arguments the caller has
-// checked (n_rows = stride = 0).  `channels` (clx_batch_create_channels, _windows): a channels mode with `n_rows` rows,
-// out_elems = n_rows * stride, and each frame's window in `windows` (null: full windows at row 0); the arguments are
-// checked here.
-int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs,
-                 const clx_frame_window* windows, size_t n_frames, size_t out_elems, uint32_t batch_flags, uint32_t mode,
-                 bool channels, uint32_t n_rows, size_t stride, clx_batch** out) {
-    if (channels) {
-        if (!ctx || !out || (!bytes && nbytes) || (!descs && n_frames) ||
-            (mode != CLX_OUT_CHANNELS_I32 && mode != CLX_OUT_CHANNELS_F32))
-            return CLX_ERR_INVALID_ARGUMENT;
-        if (n_rows == 0 || stride == 0 || stride > SIZE_MAX / 4 / n_rows) return CLX_ERR_INVALID_ARGUMENT;
-        CU(ctx, cudaSetDevice(ctx->device));
-        for (size_t i = 0; i < n_frames; i++)
-            if (!valid_window(descs[i], windows ? &windows[i] : nullptr, nbytes, n_rows, stride, mode))
-                return CLX_ERR_INVALID_ARGUMENT;
-        out_elems = (size_t)n_rows * stride;
-    }
+// The part of batch creation every mode shares, for arguments valid_frames accepted.
+int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
+                 uint32_t batch_flags, const Output& o, clx_batch** out) {
+    CU(ctx, cudaSetDevice(ctx->device));
+    const size_t stride = o.stride;
     const bool on_device = (batch_flags & CLX_BATCH_BYTES_ON_DEVICE) != 0;
     clx_batch* b = new clx_batch();
-    b->nbytes = nbytes;
-    b->buf_bytes = ((nbytes + 63) & ~(size_t)63) + 128;  // whole 64-byte TMA chunks + look-ahead
-    b->out_elems = out_elems;
+    b->out_elems = o.out_elems;
     b->n_frames = (uint32_t)n_frames;
     b->plan = make_plan(ctx, descs, n_frames);
-    b->mode = mode;
+    b->mode = o.mode;
     b->stride = stride;
     // Device descriptors in the device order (shape_order); in a channels mode each frame's window start moves to
     // `cols` (row base * stride + column) and its window to `wins`, and out_offset becomes its place in the planar
@@ -576,7 +620,7 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
     std::vector<clx_frame_desc> dev;
     std::vector<uint64_t> cols;
     std::vector<uint32_t> wins;
-    size_t planar_elems = out_elems;
+    size_t planar_elems = o.out_elems;
     if (reordered || stride) {
         dev.resize(n_frames);
         for (size_t p = 0; p < n_frames; p++) dev[p] = descs[reordered ? b->order[p] : p];
@@ -587,30 +631,19 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
         planar_elems = 0;
         for (size_t p = 0; p < n_frames; p++) {
             const size_t i = reordered ? b->order[p] : p;
-            const clx_frame_window w = windows ? windows[i] : clx_frame_window{0, 0, dev[p].block_size, 0};
+            const clx_frame_window w = o.windows ? o.windows[i] : clx_frame_window{0, 0, dev[p].block_size, 0};
             cols[p] = (uint64_t)w.row * stride + dev[p].out_offset;
             wins[p] = w.first | (w.count << 16);
             dev[p].out_offset = planar_elems;
             planar_elems += ((size_t)dev[p].n_channels * dev[p].block_size + 3) & ~(size_t)3;
         }
     }
-    cudaError_t e = cudaMalloc((void**)&b->d_bytes, b->buf_bytes);
-    if (e == cudaSuccess) e = cudaMemset(b->d_bytes, 0, b->buf_bytes);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_descs, std::max<size_t>(1, n_frames) * sizeof(clx_frame_desc));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_out, (planar_elems + 4) * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_results, std::max<size_t>(1, n_frames) * sizeof(clx_frame_result));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_need_hi, 4 * sizeof(int));
-    if (e == cudaSuccess) e = cudaMalloc(&b->d_params, clx::coop_params_bytes(b->plan, b->n_frames) + 16);
-    if (e == cudaSuccess && mode != CLX_OUT_PLANAR_I32) e = cudaMalloc(&b->d_conv, (out_elems + 8) * clx::output_elem_size(mode));
-    if (e == cudaSuccess && mode != CLX_OUT_PLANAR_I32) e = cudaMalloc((void**)&b->d_mark, std::max<size_t>(1, n_frames));
-    if (e == cudaSuccess && stride) e = cudaMemset(b->d_conv, 0, (out_elems + 8) * sizeof(int32_t));  // uncovered elements read 0
-    if (e == cudaSuccess && stride) e = cudaMalloc((void**)&b->d_cols, std::max<size_t>(1, n_frames) * sizeof(uint64_t));
-    if (e == cudaSuccess && stride) e = cudaMemcpy(b->d_cols, cols.data(), n_frames * sizeof(uint64_t), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && stride) e = cudaMalloc((void**)&b->d_wins, std::max<size_t>(1, n_frames) * sizeof(uint32_t));
-    if (e == cudaSuccess && stride) e = cudaMemcpy(b->d_wins, wins.data(), n_frames * sizeof(uint32_t), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(b->d_bytes, bytes, nbytes, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
+    cudaError_t e = b->buf.fit({nbytes, n_frames, planar_elems, o.mode, o.out_elems, true, b->plan}, false);
+    if (e == cudaSuccess && stride) e = cudaMemcpy(b->buf.cols, cols.data(), n_frames * sizeof(uint64_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && stride) e = cudaMemcpy(b->buf.wins, wins.data(), n_frames * sizeof(uint32_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(b->buf.bytes, bytes, nbytes, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
     if (e == cudaSuccess)
-        e = cudaMemcpy(b->d_descs, dev.empty() ? descs : dev.data(), n_frames * sizeof(clx_frame_desc), cudaMemcpyHostToDevice);
+        e = cudaMemcpy(b->buf.descs, dev.empty() ? descs : dev.data(), n_frames * sizeof(clx_frame_desc), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
     if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
     if (e != cudaSuccess) {
@@ -619,10 +652,7 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
     }
     if (!(ctx->flags & CLX_OPT_NO_VERIFY_CRC)) {
         if (on_device) b->device_crc = true;  // no host copy to checksum: clx_crc.cu, as part of every decode
-        else {
-            precompute_crc(ctx, bytes, descs, n_frames);
-            b->crc_ok = ctx->crc_verdict;
-        }
+        else precompute_crc(ctx, bytes, descs, n_frames, b->crc_ok);
     }
     b->h_offset.resize(n_frames);
     b->h_len.resize(n_frames);
@@ -633,8 +663,7 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
 }
 
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
-    const clx::DecodeBuffers db{b->d_bytes, b->buf_bytes, b->d_descs, b->n_frames, b->d_out, b->d_results, b->d_need_hi,
-                                b->d_params, b->mode, b->d_conv, b->d_mark, b->d_cols, b->stride, b->d_wins};
+    const clx::DecodeBuffers db = b->buf.view(b->n_frames, b->mode, b->stride);
     if (b->corpus)
         return clx::launch_crops(b->corpus->view(b->span_stride), b->crop, db, b->plan, b->device_crc, st, launches);
     return clx::launch_decode(db, b->plan, b->device_crc, st, launches);
@@ -712,13 +741,9 @@ namespace {
 // Per-frame results of the batch's last decode at the caller's frame indices, with the host-side CRC-16 verdicts.
 int read_results(clx_ctx* ctx, clx_batch* b, clx_frame_result* results) {
     if (results) {
-        if (b->order.empty()) {
-            CU(ctx, cudaMemcpy(results, b->d_results, b->n_frames * sizeof(clx_frame_result), cudaMemcpyDeviceToHost));
-        } else {
-            std::vector<clx_frame_result> dev(b->n_frames);
-            CU(ctx, cudaMemcpy(dev.data(), b->d_results, b->n_frames * sizeof(clx_frame_result), cudaMemcpyDeviceToHost));
-            for (size_t p = 0; p < b->n_frames; p++) results[b->order[p]] = dev[p];
-        }
+        std::vector<clx_frame_result> dev(b->n_frames);
+        CU(ctx, cudaMemcpy(dev.data(), b->buf.results, b->n_frames * sizeof(clx_frame_result), cudaMemcpyDeviceToHost));
+        unpermute(dev.data(), b->order, b->n_frames, results);
         if (!(ctx->flags & CLX_OPT_NO_VERIFY_CRC) && !b->device_crc) {
             std::vector<uint8_t> tmp;
             for (size_t i = 0; i < b->n_frames; i++) {
@@ -730,7 +755,7 @@ int read_results(clx_ctx* ctx, clx_batch* b, clx_frame_result* results) {
                     if (consumed < 2 || consumed > b->h_len[i]) ok = false;
                     else {
                         tmp.resize(consumed);
-                        CU(ctx, cudaMemcpy(tmp.data(), b->d_bytes + b->h_offset[i], consumed, cudaMemcpyDeviceToHost));
+                        CU(ctx, cudaMemcpy(tmp.data(), b->buf.bytes + b->h_offset[i], consumed, cudaMemcpyDeviceToHost));
                         const uint16_t stored = (uint16_t)(((uint32_t)tmp[consumed - 2] << 8) | tmp[consumed - 1]);
                         ok = clx_crc16(tmp.data(), consumed - 2) == stored;
                     }
@@ -763,17 +788,12 @@ int clx_batch_read_to(clx_ctx* ctx, clx_batch* b, void* out, size_t out_elems, c
 void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
     (void)ctx;
     if (!b) return;
-    if (b->corpus) {  // the bytes are the corpus's, or over a host corpus the batch's staging buffer
-        if (b->corpus->h_bytes) cudaFree(b->d_bytes);
+    b->buf.release();
+    if (b->corpus) {
         b->corpus->live--;
         cudaFree((void*)b->crop.requests); cudaFree(b->crop.status); cudaFree(b->crop.lengths); cudaFree(b->crop.error);
         cudaFree(b->crop.plan); cudaFree(b->crop.scan);
-    } else {
-        cudaFree(b->d_bytes);
     }
-    cudaFree(b->d_descs); cudaFree(b->d_out); cudaFree(b->d_results); cudaFree(b->d_need_hi);
-    cudaFree(b->d_params);
-    cudaFree(b->d_conv); cudaFree(b->d_mark); cudaFree(b->d_cols); cudaFree(b->d_wins);
     if (b->graph) cudaGraphExecDestroy(b->graph);
     if (b->ev_idle) cudaEventDestroy(b->ev_idle);
     if (b->ev_start) cudaEventDestroy(b->ev_start);
@@ -823,8 +843,8 @@ int clx_ctx_run_steps(clx_ctx* ctx, clx_batch** batches, size_t n_batches, uint3
     return rc;
 }
 
-void* clx_batch_device_out(clx_batch* b) { return b ? (b->mode == CLX_OUT_PLANAR_I32 ? (void*)b->d_out : b->d_conv) : nullptr; }
-void* clx_batch_device_bytes(clx_batch* b) { return b ? b->d_bytes : nullptr; }
+void* clx_batch_device_out(clx_batch* b) { return b ? (b->mode == CLX_OUT_PLANAR_I32 ? (void*)b->buf.out : b->buf.conv) : nullptr; }
+void* clx_batch_device_bytes(clx_batch* b) { return b ? b->buf.bytes : nullptr; }
 
 // Pinned host memory for callers that want true asynchronous copies.
 void* clx_host_alloc(size_t bytes) {
@@ -875,18 +895,14 @@ int clx_corpus_create(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const c
 
 int clx_corpus_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames,
                          const uint32_t* file_frames, size_t n_files, uint32_t flags, clx_corpus** out) {
-    if (!ctx || !out || (!bytes && nbytes) || (!descs && n_frames) || !file_frames) return CLX_ERR_INVALID_ARGUMENT;
+    if (!ctx || !out || !file_frames) return CLX_ERR_INVALID_ARGUMENT;
     *out = nullptr;
     if (flags & ~CLX_CORPUS_HOST) return CLX_ERR_INVALID_ARGUMENT;
     const bool host = flags & CLX_CORPUS_HOST;
     if (n_frames >= UINT32_MAX || n_files >= UINT32_MAX || file_frames[n_files] != n_frames) return CLX_ERR_INVALID_ARGUMENT;
     for (size_t i = 0; i < n_files; i++)
         if (file_frames[i + 1] < file_frames[i]) return CLX_ERR_INVALID_ARGUMENT;
-    for (size_t i = 0; i < n_frames; i++) {
-        clx_frame_desc at0 = descs[i];  // the byte-range conditions, with the frame alone in its own output
-        at0.out_offset = 0;
-        if (!valid_desc(at0, nbytes, (size_t)descs[i].n_channels * descs[i].block_size)) return CLX_ERR_INVALID_ARGUMENT;
-    }
+    if (!valid_frames(bytes, nbytes, descs, n_frames, nullptr)) return CLX_ERR_INVALID_ARGUMENT;
     // A host corpus gathers a crop's frames as one span from its first frame's start to its last frame's end.
     for (size_t i = 0; host && i < n_files; i++)
         for (size_t f = file_frames[i] + 1; f < file_frames[i + 1]; f++)
@@ -935,7 +951,7 @@ int clx_corpus_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, cons
     fd.flags |= CLX_FRAME_CRC16_VERIFIED;
     fd.out_offset = 0;
     c->descs.push_back(fd);
-    c->buf_bytes = ((nbytes + filler_len + 63) & ~(size_t)63) + 128;  // whole 64-byte TMA chunks + look-ahead
+    c->buf_bytes = padded_bytes(nbytes + filler_len);
     cudaError_t e = cudaSuccess;
     if (host) {  // the crop batches stage what they decode; the filler frame is copied from here into each of them
         e = cudaHostAlloc((void**)&c->h_bytes, c->buf_bytes, cudaHostAllocMapped);
@@ -987,7 +1003,7 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
     if (!out) return CLX_ERR_INVALID_ARGUMENT;
     *out = nullptr;
     if (!ctx || !corpus || n_crops == 0 || num_frames == 0 || n_crops >= (1u << 30) ||
-        (mode != CLX_OUT_CHANNELS_I32 && mode != CLX_OUT_CHANNELS_F32) || (mode == CLX_OUT_CHANNELS_F32 && corpus->max_bps > 24))
+        !is_channels(mode) || (mode == CLX_OUT_CHANNELS_F32 && corpus->max_bps > 24))
         return CLX_ERR_INVALID_ARGUMENT;
     const size_t S = clx_crop_frames_bound(corpus->descs.data(), corpus->n_frames, corpus->file_frames.data(),
                                            corpus->n_files, num_frames);
@@ -997,35 +1013,22 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
     if (S == 0 || S > UINT32_MAX / n_crops || num_frames > (SIZE_MAX / 4 - 8) / (rows + C)) return CLX_ERR_INVALID_ARGUMENT;
     const size_t slots = n_crops * S;
     if (slots > (SIZE_MAX / 4 - 8) / slot_elems) return CLX_ERR_INVALID_ARGUMENT;
-    // Over a host corpus: crop b's span at b * span_stride + (its start & 15), the filler frame after the last span,
-    // then whole 64-byte TMA chunks + look-ahead (DecodeBuffers' contract).
-    size_t span_stride = 0, staging = 0;
+    // Over a host corpus, the batch's own frame bytes: crop b's span at b * span_stride + (its start & 15), then the
+    // filler frame after the last span.
+    size_t span_stride = 0;
     const size_t filler_len = clx::filler_frame(nullptr, 0);
     if (corpus->h_bytes) {
         const size_t span = clx_crop_bytes_bound(corpus->descs.data(), corpus->n_frames, corpus->file_frames.data(),
                                                  corpus->n_files, num_frames);
         span_stride = (span + 15 + 15) & ~(size_t)15;
         if (span_stride > (SIZE_MAX / 2) / n_crops) return CLX_ERR_INVALID_ARGUMENT;
-        staging = ((n_crops * span_stride + filler_len + 63) & ~(size_t)63) + 128;
     }
     CU(ctx, cudaSetDevice(ctx->device));
     clx_batch* b = new clx_batch();
     b->corpus = corpus;
     corpus->live++;
-    b->d_bytes = corpus->d_bytes;
-    b->nbytes = corpus->nbytes;
-    b->buf_bytes = corpus->buf_bytes;
+    if (!corpus->h_bytes) b->buf.borrow(corpus->d_bytes, corpus->buf_bytes);
     b->span_stride = span_stride;
-    cudaError_t e = cudaSuccess;
-    if (corpus->h_bytes) {
-        b->nbytes = n_crops * span_stride + filler_len;
-        b->buf_bytes = staging;
-        e = cudaMalloc((void**)&b->d_bytes, staging);
-        if (e == cudaSuccess) e = cudaMemset(b->d_bytes, 0, staging);
-        if (e == cudaSuccess)
-            e = cudaMemcpy(b->d_bytes + n_crops * span_stride, corpus->h_bytes + corpus->nbytes, filler_len,
-                           cudaMemcpyHostToDevice);
-    }
     b->n_frames = (uint32_t)slots;
     b->out_elems = rows * num_frames;
     b->plan = plan;
@@ -1039,17 +1042,12 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
     cb.n_slots = (uint32_t)slots;
     cb.L = num_frames;
     cb.slot_elems = slot_elems;
-    const size_t conv_elems = (rows + C) * num_frames + 8;  // the output, C trash rows for the unused slots, vector slack
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_descs, slots * sizeof(clx_frame_desc));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_out, (slots * slot_elems + 4) * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_results, slots * sizeof(clx_frame_result));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_need_hi, 4 * sizeof(int));
-    if (e == cudaSuccess) e = cudaMalloc(&b->d_params, clx::coop_params_bytes(plan, b->n_frames) + 16);
-    if (e == cudaSuccess) e = cudaMalloc(&b->d_conv, conv_elems * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMemset(b->d_conv, 0, conv_elems * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_mark, slots);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_cols, slots * sizeof(uint64_t));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_wins, slots * sizeof(uint32_t));
+    // the output plus C trash rows for the unused slots
+    cudaError_t e = b->buf.fit({n_crops * span_stride + filler_len, slots, slots * slot_elems, mode, (rows + C) * num_frames,
+                                true, plan}, false);
+    if (e == cudaSuccess && corpus->h_bytes)
+        e = cudaMemcpy(b->buf.bytes + n_crops * span_stride, corpus->h_bytes + corpus->nbytes, filler_len,
+                       cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMalloc((void**)&cb.requests, n_crops * sizeof(clx_crop_request));
     if (e == cudaSuccess) e = cudaMemset((void*)cb.requests, 0, n_crops * sizeof(clx_crop_request));
     if (e == cudaSuccess) e = cudaMalloc((void**)&cb.status, n_crops * sizeof(int32_t));

@@ -28,7 +28,7 @@ from ._lib import (FrameDesc, FrameResult, FrameWindow, OPT_NO_VERIFY_CRC, OPT_G
 __all__ = ["Error", "Block", "FrameReader", "FlacReader", "FlacReaderOptions", "StreamInfo", "Context", "DeviceBatch",
            "parse_frame_header", "demux_frames", "open_stream", "ogg_frames", "mp4_frames", "status_str", "DESC_DTYPE", "RESULT_DTYPE", "load", "plan_columns",
            "WINDOW_DTYPE", "index", "FlacIndex", "IndexedFile", "load_crops", "plan_range", "frame_starts", "Corpus",
-           "CropBatch"]
+           "CropBatch", "PackedBatch"]
 
 # numpy views of the C structs (same layout; asserted below)
 DESC_DTYPE = np.dtype([
@@ -1022,6 +1022,21 @@ class Corpus:
         reads the selected crops' span bytes (about span bytes x batch) from host memory over PCIe."""
         return CropBatch(self, batch, num_frames, dtype)
 
+    def packed_frames_bound(self, max_excerpts: int, max_samples: int) -> int:
+        """clx_packed_frames_bound: the most frames the excerpts of one packed call can overlap together."""
+        return int(self.ctx._L.clx_packed_frames_bound(self.descs.ctypes.data, self.descs.size, self.file_frames.ctypes.data,
+                                                       len(self.index), int(max_excerpts), int(max_samples)))
+
+    def packed_bytes_bound(self, max_excerpts: int, max_samples: int) -> int:
+        """clx_packed_bytes_bound: the staging bytes of a packed batch over a host corpus."""
+        return int(self.ctx._L.clx_packed_bytes_bound(self.descs.ctypes.data, self.descs.size, self.file_frames.ctypes.data,
+                                                      len(self.index), int(max_excerpts), int(max_samples)))
+
+    def packed(self, max_excerpts: int, max_samples: int, dtype=None) -> "PackedBatch":
+        """A PackedBatch of up to `max_excerpts` excerpts laid out along `max_samples` columns; its CUDA graph is
+        instantiated here."""
+        return PackedBatch(self, max_excerpts, max_samples, dtype)
+
     def close(self):
         """Frees the corpus's copy of the bytes and its index; raises Error while a CropBatch of the corpus is alive."""
         if getattr(self, "_h", None) and getattr(self.ctx, "_h", None):
@@ -1120,6 +1135,128 @@ class CropBatch:
                 raise ValueError(f"crop {b}: file index {fi} out of range")
             raise ValueError(f"crop {b}: offset {o} outside file {fi} ({self.corpus.index[fi].length} samples)")
         raise Error(st, f"file {fi}, crop {b}")
+
+    def kernel_ms(self) -> float:
+        """Device time of the last call's graph (CUDA events), planner and status pass included."""
+        return self._batch.kernel_ms()
+
+
+def _request_column(x, n: int | None, what: str):
+    """A request column as an int64 CUDA tensor (integers only; CPU values are copied through pinned memory)."""
+    import torch
+    if isinstance(x, torch.Tensor):
+        if x.dtype.is_floating_point or x.dtype.is_complex or x.dtype == torch.bool:
+            raise TypeError(f"{what} must hold integers")
+        t = x.reshape(-1)
+    else:
+        t = torch.from_numpy(np.asarray(x, dtype=np.int64).reshape(-1))
+    if n is not None and t.numel() != n:
+        raise ValueError(f"{what}: {t.numel()} values for {n} files")
+    if not t.is_cuda:
+        t = t.to(torch.int64).pin_memory().to("cuda", non_blocking=True)
+    return t
+
+
+class PackedBatch:
+    """Whole files or excerpts of different lengths of a Corpus's files, packed along the columns of one [C, T] CUDA
+    tensor per call (clx_batch_create_packed), the layout of load(): excerpt b starts at column starts[b], each start a
+    multiple of 4, start_{b+1} = start_b + round_up_4(n_b).  As for CropBatch, the frames, windows and columns are planned
+    on the device inside the batch's CUDA graph, so a call is a few small device copies and one graph launch, and the
+    requests may be CUDA tensors.  C is the corpus's largest channel count, T = max_samples.
+
+    Excerpt b is samples [offsets[b], offsets[b] + n_b) of file files[b], n_b = min(lengths[b], N - offsets[b]) (to the
+    file's end for a length of -1, the default; offsets default to 0).  Channel c goes to row c; every other element of
+    the [C, T] output reads 0.  An excerpt whose columns would pass T does not fit: it gets length 0 and status 90, like
+    an invalid request (the excerpts that fit are a prefix of the valid ones).  `out`, `starts`, `lengths` and `status`
+    are views of the batch's own buffers, overwritten by the next call; the next call waits for what torch's current
+    stream has enqueued before it.  A float32 batch is refused when any frame of the corpus has more than 24 bits.
+    Memory: C x (T + the trash columns) output elements and a planar scratch of the corpus's largest frame for each of
+    packed_frames_bound(max_excerpts, T) slots; over a host corpus also a staging buffer of packed_bytes_bound() bytes,
+    and each call reads the selected spans over PCIe."""
+
+    def __init__(self, corpus: Corpus, max_excerpts: int, max_samples: int, dtype=None):
+        import torch
+        dtype = _torch_dtype(dtype)
+        self.corpus, self.ctx = corpus, corpus.ctx
+        self.max_excerpts, self.max_samples, self.dtype = int(max_excerpts), int(max_samples), dtype
+        if self.max_excerpts < 1 or self.max_samples < 1:
+            raise ValueError("max_excerpts and max_samples must be >= 1")
+        mode = _channels_mode(dtype)
+        L = self.ctx._L
+        h = C.c_void_p()
+        _check(L.clx_batch_create_packed(self.ctx._h, corpus._h, self.max_excerpts, self.max_samples, mode, C.byref(h)),
+               self.ctx)
+        self._batch = _Batch(self.ctx, h, keep=corpus)
+        self.channels = corpus.channels
+        self.stride = int(L.clx_batch_packed_stride(h))
+        B, view = self.max_excerpts, self._batch.tensor
+        self.out = view(L.clx_batch_device_out(h), (self.channels, self.stride),
+                        "<f4" if mode == OUT_CHANNELS_F32 else "<i4")[:, :self.max_samples]
+        self._starts = view(L.clx_batch_packed_starts(h), (B,), "<i8")
+        self._lengths = view(L.clx_batch_crop_lengths(h), (B,), "<i8")
+        self._status = view(L.clx_batch_crop_status(h), (B,), "<i4")
+        self._requests = view(L.clx_batch_packed_requests(h), (B, 3), "<i8")  # {u32 file, u32 reserved}, offset, length
+        self._count = view(L.clx_batch_packed_count(h), (1,), "<i4")
+        self._error = view(L.clx_batch_crop_error(h), (1,), "<i8")
+        self._stream = torch.cuda.ExternalStream(L.clx_ctx_stream(self.ctx._h, 0))
+        self._n = 0
+
+    @property
+    def status(self):
+        """Each excerpt's status of the last call (an int32 CUDA tensor view)."""
+        return self._status[:self._n]
+
+    def __call__(self, files, offsets=None, lengths=None, check: bool = True):
+        """Decodes excerpt b = samples [offsets[b], offsets[b] + lengths[b]) of file files[b], cut at the file's end,
+        for each of the n <= max_excerpts files.  Returns (out [C, T], starts [n] int64, lengths [n] int64), on the GPU.
+        The requests are copied and the count set on torch's current stream, the batch's stream waits for it and torch's
+        stream waits for the decode: nothing syncs with the host unless `check`.  check=True syncs once and raises, for
+        the first excerpt in order that has one: ValueError for an invalid request or an excerpt that does not fit, else
+        Error(status, "file i, excerpt b") for a failed frame or what follows a file's unconfirmed last frame.  With
+        check=False nothing is raised and `status` holds each excerpt's outcome (90 for an invalid or non-fitting one)."""
+        import torch
+        files = _request_column(files, None, "files")
+        n = files.numel()
+        if n > self.max_excerpts:
+            raise ValueError(f"{n} excerpts for a batch of at most {self.max_excerpts}")
+        req = self._requests[:n]
+        req[:, 0].copy_(files)
+        if offsets is None:
+            req[:, 1].zero_()
+        else:
+            req[:, 1].copy_(_request_column(offsets, n, "offsets"))
+        if lengths is None:
+            req[:, 2].fill_(-1)
+        else:
+            req[:, 2].copy_(_request_column(lengths, n, "lengths"))
+        self._count.fill_(n)
+        self._n = n
+        self._stream.wait_stream(torch.cuda.current_stream())
+        self._batch.decode(0)
+        torch.cuda.current_stream().wait_stream(self._stream)
+        if check:
+            self._raise()
+        return self.out, self._starts[:n], self._lengths[:n]
+
+    def _raise(self):
+        err = int(self._error.item()) & ((1 << 64) - 1)  # the one sync
+        if err == (1 << 64) - 1:
+            return
+        kind, b, st = err >> 62, (err >> 32) & ((1 << 30) - 1), err & 0xffffffff
+        st = st - (1 << 32) if st >= 1 << 31 else st
+        fi, o, ln = (int(v) for v in self._requests[b].tolist())
+        if kind == 0:
+            if not 0 <= fi < len(self.corpus.index):
+                raise ValueError(f"excerpt {b}: file index {fi} out of range")
+            N = self.corpus.index[fi].length
+            if not 0 <= o <= N:
+                raise ValueError(f"excerpt {b}: offset {o} outside file {fi} ({N} samples)")
+            if ln == 0 or ln < -1:
+                raise ValueError(f"excerpt {b}: length {ln} (must be >= 1, or -1 for the rest of the file)")
+            start = int(self._starts[b].item())
+            n = N - o if ln == -1 else min(ln, N - o)
+            raise ValueError(f"excerpt {b}: needs columns [{start}, {start + n}), past max_samples {self.max_samples}")
+        raise Error(st, f"file {fi}, excerpt {b}")
 
     def kernel_ms(self) -> float:
         """Device time of the last call's graph (CUDA events), planner and status pass included."""

@@ -102,6 +102,13 @@ SYMBOLS = {
     "clx_batch_crop_lengths": (_vp, [_vp]),
     "clx_batch_crop_error": (_vp, [_vp]),
     "clx_crop_filler_frame": (_sz, [_vp, _sz]),
+    "clx_batch_create_packed": (C.c_int, [_vp, _vp, _sz, _sz, C.c_uint32, C.POINTER(_vp)]),
+    "clx_packed_frames_bound": (_sz, [_vp, _sz, _vp, _sz, _sz, _sz]),
+    "clx_packed_bytes_bound": (_sz, [_vp, _sz, _vp, _sz, _sz, _sz]),
+    "clx_batch_packed_requests": (_vp, [_vp]),
+    "clx_batch_packed_count": (_vp, [_vp]),
+    "clx_batch_packed_starts": (_vp, [_vp]),
+    "clx_batch_packed_stride": (_sz, [_vp]),
     "clx_batch_decode": (C.c_int, [_vp, _vp, C.c_uint32]),
     "clx_batch_sync": (C.c_int, [_vp, _vp]),
     "clx_batch_read": (C.c_int, [_vp, _vp, _vp, _sz, _vp]),

@@ -223,9 +223,14 @@ struct clx_batch {
     // Crop batches (clx_batch_create_crops): buf.bytes is the corpus's, not the batch's; the planner writes buf.descs,
     // buf.cols and buf.wins in every decode (clx_crops.cu).  Over a host corpus, buf.bytes is the batch's own staging
     // buffer: n_crops spans of span_stride bytes, then the filler frame.
+    // Packed batches (clx_batch_create_packed) are crop batches with `packed` set: crop holds their per-excerpt plan,
+    // status, lengths, error word and slot scan, and over a host corpus span_stride is the staging bound, after which
+    // the filler frame is staged.
     clx_corpus* corpus = nullptr;
     clx::CropBuffers crop{};
     uint64_t span_stride = 0;
+    bool is_packed = false;
+    clx::PackedBuffers packed{};
 };
 
 struct clx_corpus {
@@ -243,7 +248,7 @@ struct clx_corpus {
     std::vector<clx_frame_desc> descs;  // host copy, the filler frame last
     std::vector<uint32_t> file_frames;
     uint32_t channels = 1, max_bps = 0;
-    int live = 0;  // crop batches of this corpus
+    int live = 0;  // crop and packed batches of this corpus
     clx::CropCorpus view(uint64_t span_stride) const {
         return {d_descs, d_starts, d_file_frames, d_file_len, d_file_ch, d_file_tail, n_files, n_frames, d_host,
                 d_host ? span_stride : 0};
@@ -664,6 +669,9 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
 
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
     const clx::DecodeBuffers db = b->buf.view(b->n_frames, b->mode, b->stride);
+    if (b->corpus && b->is_packed)
+        return clx::launch_packed(b->corpus->view(b->span_stride), b->crop, b->packed, db, b->plan, b->device_crc, st,
+                                  launches);
     if (b->corpus)
         return clx::launch_crops(b->corpus->view(b->span_stride), b->crop, db, b->plan, b->device_crc, st, launches);
     return clx::launch_decode(db, b->plan, b->device_crc, st, launches);
@@ -793,6 +801,8 @@ void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
         b->corpus->live--;
         cudaFree((void*)b->crop.requests); cudaFree(b->crop.status); cudaFree(b->crop.lengths); cudaFree(b->crop.error);
         cudaFree(b->crop.plan); cudaFree(b->crop.scan);
+        cudaFree((void*)b->packed.requests); cudaFree((void*)b->packed.count); cudaFree(b->packed.starts);
+        cudaFree(b->packed.stage); cudaFree(b->packed.chunks); cudaFree(b->packed.end);
     }
     if (b->graph) cudaGraphExecDestroy(b->graph);
     if (b->ev_idle) cudaEventDestroy(b->ev_idle);
@@ -998,6 +1008,39 @@ int clx_corpus_destroy(clx_ctx* ctx, clx_corpus* corpus) {
 
 size_t clx_corpus_device_bytes(const clx_corpus* corpus) { return corpus ? corpus->device_bytes : 0; }
 
+}  // extern "C"
+
+namespace {
+template <typename T>
+cudaError_t device_zeros(T*& p, size_t n) {
+    cudaError_t e = cudaMalloc((void**)&p, n * sizeof(T));
+    return e == cudaSuccess ? cudaMemset((void*)p, 0, n * sizeof(T)) : e;
+}
+template <typename T>
+cudaError_t device_zeros(const T*& p, size_t n) {
+    T* q = nullptr;
+    const cudaError_t e = device_zeros(q, n);
+    p = q;
+    return e;
+}
+
+// The per-excerpt buffers every crop or packed batch's planner writes (all but the requests), and its timing events.
+cudaError_t alloc_planner(clx_batch* b, size_t n) {
+    clx::CropBuffers& cb = b->crop;
+    cudaError_t e = device_zeros(cb.status, n);
+    if (e == cudaSuccess) e = device_zeros(cb.lengths, n);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.error, sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMemset(cb.error, 0xff, sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.plan, n * sizeof(clx::CropPlan));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.scan, (n + 1) * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
+    return e;
+}
+}  // namespace
+
+extern "C" {
+
 int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, size_t num_frames, uint32_t mode,
                            clx_batch** out) {
     if (!out) return CLX_ERR_INVALID_ARGUMENT;
@@ -1048,18 +1091,8 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
     if (e == cudaSuccess && corpus->h_bytes)
         e = cudaMemcpy(b->buf.bytes + n_crops * span_stride, corpus->h_bytes + corpus->nbytes, filler_len,
                        cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.requests, n_crops * sizeof(clx_crop_request));
-    if (e == cudaSuccess) e = cudaMemset((void*)cb.requests, 0, n_crops * sizeof(clx_crop_request));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.status, n_crops * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMemset(cb.status, 0, n_crops * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.lengths, n_crops * sizeof(int64_t));
-    if (e == cudaSuccess) e = cudaMemset(cb.lengths, 0, n_crops * sizeof(int64_t));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.error, sizeof(unsigned long long));
-    if (e == cudaSuccess) e = cudaMemset(cb.error, 0xff, sizeof(unsigned long long));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.plan, n_crops * sizeof(clx::CropPlan));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.scan, (n_crops + 1) * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
+    if (e == cudaSuccess) e = device_zeros(cb.requests, n_crops);
+    if (e == cudaSuccess) e = alloc_planner(b, n_crops);
     if (e != cudaSuccess) {
         clx_batch_destroy(ctx, b);
         return cuda_fail(ctx, e, "clx_batch_create_crops");
@@ -1073,6 +1106,82 @@ void* clx_batch_crop_requests(clx_batch* b) { return b && b->corpus ? (void*)b->
 void* clx_batch_crop_status(clx_batch* b) { return b && b->corpus ? (void*)b->crop.status : nullptr; }
 void* clx_batch_crop_lengths(clx_batch* b) { return b && b->corpus ? (void*)b->crop.lengths : nullptr; }
 void* clx_batch_crop_error(clx_batch* b) { return b && b->corpus ? (void*)b->crop.error : nullptr; }
+
+int clx_batch_create_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpts, size_t max_samples, uint32_t mode,
+                            clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (!ctx || !corpus || max_excerpts == 0 || max_samples == 0 || max_excerpts >= (1u << 30) ||
+        max_samples > SIZE_MAX / 16 || !is_channels(mode) || (mode == CLX_OUT_CHANNELS_F32 && corpus->max_bps > 24))
+        return CLX_ERR_INVALID_ARGUMENT;
+    const clx_frame_desc* descs = corpus->descs.data();
+    const uint32_t* ff = corpus->file_frames.data();
+    const size_t S = clx_packed_frames_bound(descs, corpus->n_frames, ff, corpus->n_files, max_excerpts, max_samples);
+    uint32_t largest = 0;  // block size, the filler frame's included (the unused slots decode it into the trash)
+    for (const clx_frame_desc& d : corpus->descs) largest = std::max<uint32_t>(largest, d.block_size);
+    const size_t T4 = (max_samples + 3) & ~(size_t)3, W = (std::min<size_t>(max_samples, largest) + 3) & ~(size_t)3;
+    const size_t C = corpus->channels, stride = T4 + W;
+    const clx::Plan plan = make_plan(ctx, descs, corpus->descs.size());
+    const size_t slot_elems = ((size_t)plan.max_frame_elems + 3) & ~(size_t)3;
+    if (S == 0 || S >= UINT32_MAX || stride > (SIZE_MAX / 4 - 8) / C || S > (SIZE_MAX / 4 - 8) / slot_elems)
+        return CLX_ERR_INVALID_ARGUMENT;
+    // Over a host corpus, the batch's own frame bytes: the excerpts' spans packed from 0 (at most the bytes bound), then
+    // the filler frame.
+    size_t span_stride = 0, chunks = 0;
+    const size_t filler_len = clx::filler_frame(nullptr, 0);
+    if (corpus->h_bytes) {
+        span_stride = clx_packed_bytes_bound(descs, corpus->n_frames, ff, corpus->n_files, max_excerpts, max_samples);
+        if (span_stride > SIZE_MAX / 2) return CLX_ERR_INVALID_ARGUMENT;
+        chunks = span_stride / (16 * 1024) + max_excerpts;  // ceil(span / GATHER_CHUNK) per excerpt, every span together
+    }
+    CU(ctx, cudaSetDevice(ctx->device));
+    clx_batch* b = new clx_batch();
+    b->corpus = corpus;
+    corpus->live++;
+    b->is_packed = true;
+    if (!corpus->h_bytes) b->buf.borrow(corpus->d_bytes, corpus->buf_bytes);
+    b->span_stride = span_stride;
+    b->n_frames = (uint32_t)S;
+    b->out_elems = C * stride;
+    b->plan = plan;
+    b->mode = mode;
+    b->stride = stride;
+    b->device_crc = !(ctx->flags & CLX_OPT_NO_VERIFY_CRC);
+    clx::CropBuffers& cb = b->crop;
+    cb.n_crops = (uint32_t)max_excerpts;
+    cb.C = (uint32_t)C;
+    cb.S = (uint32_t)S;
+    cb.n_slots = (uint32_t)S;
+    cb.L = stride;
+    cb.slot_elems = slot_elems;
+    clx::PackedBuffers& pb = b->packed;
+    pb.T = max_samples;
+    pb.W = W;
+    pb.max_chunks = (uint32_t)std::min<size_t>(std::max<size_t>(chunks, 1), 1u << 20);
+    // the output with its trash columns, zeroed here: afterwards every call zeroes what it must
+    cudaError_t e = b->buf.fit({span_stride + filler_len, S, S * slot_elems, mode, C * stride, true, plan}, false);
+    if (e == cudaSuccess && corpus->h_bytes)
+        e = cudaMemcpy(b->buf.bytes + span_stride, corpus->h_bytes + corpus->nbytes, filler_len, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = device_zeros(pb.requests, max_excerpts);
+    if (e == cudaSuccess) e = device_zeros(pb.count, 1);
+    if (e == cudaSuccess) e = device_zeros(pb.starts, max_excerpts);
+    if (e == cudaSuccess) e = device_zeros(pb.stage, max_excerpts);
+    if (e == cudaSuccess) e = device_zeros(pb.chunks, max_excerpts + 1);
+    if (e == cudaSuccess) e = device_zeros(pb.end, 2);
+    if (e == cudaSuccess) e = alloc_planner(b, max_excerpts);
+    if (e != cudaSuccess) {
+        clx_batch_destroy(ctx, b);
+        return cuda_fail(ctx, e, "clx_batch_create_packed");
+    }
+    build_graph(ctx, b);
+    *out = b;
+    return CLX_OK;
+}
+
+void* clx_batch_packed_requests(clx_batch* b) { return b && b->is_packed ? (void*)b->packed.requests : nullptr; }
+void* clx_batch_packed_count(clx_batch* b) { return b && b->is_packed ? (void*)b->packed.count : nullptr; }
+void* clx_batch_packed_starts(clx_batch* b) { return b && b->is_packed ? (void*)b->packed.starts : nullptr; }
+size_t clx_batch_packed_stride(clx_batch* b) { return b && b->is_packed ? b->stride : 0; }
 
 }  // extern "C"
 

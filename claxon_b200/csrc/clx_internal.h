@@ -127,6 +127,21 @@ struct CropBuffers {
     uint64_t L;       // num_frames: the row length
     uint64_t slot_elems;
 };
+// Packed batches (clx_batch_create_packed) keep their per-excerpt plan, status, lengths, error word and slot scan in a
+// CropBuffers (n_crops = max_excerpts, S = n_slots = the slot bound, L = the row stride), and the rest here.  Over a
+// host corpus the staging buffer holds each excerpt's span at stage[b], the scan of span bytes + 15 moved up to the
+// span start's residue mod 16, and the filler frame at CropCorpus::span_stride (the staging bound).
+struct PackedBuffers {
+    const clx_packed_request* requests;
+    const uint32_t* count;  // excerpts this call uses (device, written by the caller)
+    int64_t* starts;        // each excerpt's first column
+    uint64_t* stage;        // host corpus: where each excerpt's span starts in the staging buffer
+    uint32_t* chunks;       // n + 1: exclusive scan of each span's gather chunks, then the total
+    uint64_t* end;          // [0]: this call's end column, [1]: the previous call's
+    uint64_t T;             // max_samples: the columns users see
+    uint64_t W;             // trash columns after round_up_4(T)
+    uint32_t max_chunks;    // the gather's grid
+};
 // Filler frame: 1 channel, 16 bits, block size 192, CONSTANT 0.  Writes it if cap suffices; returns its length.
 size_t filler_frame(uint8_t* out, size_t cap);
 // The crop batch's launch sequence: planner (count, scan, the gather of a host corpus, emit, zero-fill), launch_decode
@@ -134,6 +149,9 @@ size_t filler_frame(uint8_t* out, size_t cap);
 // over a host corpus db.bytes is the staging buffer the gather writes.
 cudaError_t launch_crops(const CropCorpus& cc, const CropBuffers& cb, const DecodeBuffers& db, const Plan& plan, bool crc,
                          cudaStream_t stream, uint64_t* launches);
+// The packed batch's launch sequence, of the same shape (clx_crops.cu).
+cudaError_t launch_packed(const CropCorpus& cc, const CropBuffers& cb, const PackedBuffers& pb, const DecodeBuffers& db,
+                          const Plan& plan, bool crc, cudaStream_t stream, uint64_t* launches);
 #ifdef CLX_EXPERIMENT
 extern int g_exp_which;  // measurement builds only: bit 0 = index pass, bit 1 = decode pass of LanePerFrame
 extern int g_exp_dyn_smem;

@@ -347,6 +347,52 @@ void* clx_batch_crop_error(clx_batch* b);
 /* The frame a crop batch decodes in its unused slots (1 channel, 16 bits, 192 samples of CONSTANT 0, valid CRC-8 and
  * CRC-16), for inspection: writes it into out if cap suffices and returns its length in bytes.  Host only. */
 size_t clx_crop_filler_frame(uint8_t* out, size_t cap);
+/* Packed batches: whole files or excerpts of different lengths of a corpus, one after another along the columns of one
+ * [C, max_samples] output (load()'s layout), planned on the device like a crop batch.  A call: write `count` requests
+ * into clx_batch_packed_requests and the count into clx_batch_packed_count (device memory), clx_batch_decode.
+ *
+ * Excerpt b < count is samples [offset, offset + n_b) of its file, n_b = min(length, N - offset) (N - offset for a
+ * length of -1), N the file's length.  Columns: start_0 = 0, start_{b+1} = start_b + round_up_4(n_b).  A request with
+ * file >= n_files, reserved != 0, offset < 0 or > N, length 0 or below -1 is invalid and takes 0 columns; an excerpt
+ * with start_b + n_b > max_samples does not fit.  Both get status CLX_ERR_INVALID_ARGUMENT, length 0 and no frames
+ * (starts only grow, so the excerpts that fit are a prefix of the valid ones).  Channel c of excerpt b goes to row c,
+ * columns [start_b, start_b + n_b); every other element of [C, max_samples] is 0 after the call (the batch keeps the
+ * previous call's end column and zeroes only what lies between the two ends, never the whole output).  Status, lengths
+ * and the error word: clx_batch_crop_status / _lengths / _error, per excerpt as for crop batches (kind 0 covers invalid
+ * and non-fitting excerpts).
+ * Output: C rows of clx_batch_packed_stride elements, C the corpus's largest channel count; stride = round_up_4(
+ * max_samples) + W, the W = round_up_4(min(max_samples, the largest block size of the corpus and the filler frame))
+ * columns after round_up_4(max_samples) take the unused slots.  Memory: C * stride output elements and, per slot, a
+ * planar scratch of the corpus's largest frame, slots = clx_packed_frames_bound; over a host corpus also a staging
+ * buffer of clx_packed_bytes_bound bytes plus the filler frame and slack.
+ * CLX_ERR_INVALID_ARGUMENT for: max_excerpts 0 or 2^30 or more, max_samples 0, slots of 2^32 or more, sizes that
+ * overflow, a mode other than the two channels modes, F32 with a frame above 24 bits. */
+typedef struct clx_packed_request {
+    uint32_t file;     /* index of the file in the corpus */
+    uint32_t reserved; /* 0 */
+    int64_t offset;    /* first sample, 0 .. the file's length */
+    int64_t length;    /* >= 1, or -1: to the end of the file */
+} clx_packed_request;
+int clx_batch_create_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpts, size_t max_samples, uint32_t mode,
+                            clx_batch** out);
+/* The most frames the excerpts that fit can overlap together: with k = min(max_excerpts, max_samples) and m the smallest
+ * block size among the frames that are not the last of their file, floor((max_samples - 2k) / m) + 2k (rounded down),
+ * at most k times the frames of the largest file; k when no file has two frames.  Host only.  0 for a bad file_frames or
+ * a zero argument. */
+size_t clx_packed_frames_bound(const clx_frame_desc* descs, size_t n_frames, const uint32_t* file_frames, size_t n_files,
+                               size_t max_excerpts, size_t max_samples);
+/* The staging bytes of a packed batch over a host corpus: clx_packed_frames_bound times the largest per-frame byte
+ * advance (a frame's distance to the next frame of its file, or its byte_len when that is larger or it is the last), plus
+ * 16 per excerpt for alignment.  SIZE_MAX if that overflows.  Host only.  0 for a bad file_frames or a zero argument. */
+size_t clx_packed_bytes_bound(const clx_frame_desc* descs, size_t n_frames, const uint32_t* file_frames, size_t n_files,
+                              size_t max_excerpts, size_t max_samples);
+/* Device pointers of a packed batch (NULL for other batches): max_excerpts requests (zeroed at creation); one uint32, how
+ * many of them a call uses (0 at creation); max_excerpts int64 column starts, written by each call.  The row stride of
+ * the output in elements (0 for other batches). */
+void* clx_batch_packed_requests(clx_batch* b);
+void* clx_batch_packed_count(clx_batch* b);
+void* clx_batch_packed_starts(clx_batch* b);
+size_t clx_batch_packed_stride(clx_batch* b);
 int clx_batch_decode(clx_ctx* ctx, clx_batch* b, uint32_t stream_index); /* async on an internal stream */
 int clx_batch_sync(clx_ctx* ctx, clx_batch* b);
 /* Planar batches only (CLX_ERR_INVALID_ARGUMENT for any other mode). */

@@ -331,6 +331,11 @@ class _Batch:
         if getattr(self, "h", None) and getattr(self.ctx, "_h", None):
             self.ctx._L.clx_batch_destroy(self.ctx._h, self.h)
         self.h = None
+        if getattr(self.keep, "_close_pending", False):  # (see Corpus.__del__)
+            try:
+                self.keep.close()
+            except Exception:  # another batch of it is still alive: the last one closes it
+                pass
 
     def __del__(self):
         try:
@@ -970,7 +975,8 @@ class Corpus:
     memory the GPU reads directly, and only the frame index (about 48 bytes per frame) on the GPU: for corpora that
     should not take GPU memory from the model.  Every call of a crop batch of a host corpus then copies the frames its
     crops selected over PCIe first (about the crops' span bytes x B per call), so it is slower than over a device
-    corpus; the results are the same.  `device_bytes` is the GPU memory the corpus holds."""
+    corpus; the results are the same.  `device_bytes` is the GPU memory the corpus holds.  For data-parallel jobs,
+    Corpus.share() and Corpus.attach() give a host corpus whose pinned bytes exist once per machine (memory "shared")."""
 
     def __init__(self, index: FlacIndex, ctx: Context | None = None, memory: str = "device"):
         if memory not in ("device", "host"):
@@ -1037,17 +1043,169 @@ class Corpus:
         instantiated here."""
         return PackedBatch(self, max_excerpts, max_samples, dtype)
 
+    @classmethod
+    def share(cls, index: FlacIndex, path, ctx: Context | None = None) -> "Corpus":
+        """Writes `index` as a corpus image at `path` (clx_corpus_image_write) and attaches it (Corpus.attach).
+
+        An image holds the frame index and the compressed bytes of a host corpus in one file that every process and
+        GPU of a machine can attach, so a data-parallel job pins the bytes once per machine instead of once per rank.
+        Put it on a tmpfs such as /dev/shm: its pages are the pinned memory.  Each file's bytes are copied straight
+        from its own buffer (the index's memory map), with no concatenated copy; the trailing-bytes verdicts are taken
+        once here.  The image is written under a temporary name in the same directory and linked to `path` when
+        complete, so attachers see all of it or nothing; its size is reserved first (posix_fallocate), so a tmpfs that
+        is too small raises OSError before anything is copied.  A `path` that exists is refused (FileExistsError).
+
+        The usual pattern, one process per GPU::
+
+            if rank == 0:
+                corpus = Corpus.share(index, "/dev/shm/train.clxc")
+            barrier()
+            if rank != 0:
+                corpus = Corpus.attach("/dev/shm/train.clxc")
+            barrier()
+            if rank == 0:
+                os.unlink("/dev/shm/train.clxc")  # optional: the pages live until the last mapping goes
+
+        Removing the file is the caller's job; the memory is freed when it is unlinked and the last process has
+        closed its corpus (or exited)."""
+        import mmap
+        import os
+        import secrets
+        ctx = ctx or default_context()
+        path = os.fspath(path)
+        if os.path.lexists(path):
+            raise FileExistsError(17, "corpus image exists", path)
+        L, n = ctx._L, len(index)
+        datas = [_as_u8(f.data) for f in index.files]
+        descs = (np.ascontiguousarray(np.concatenate([f.descs for f in index.files]), dtype=DESC_DTYPE) if n else
+                 np.zeros(0, dtype=DESC_DTYPE))
+        file_frames = np.concatenate([[0], np.cumsum([f.descs.size for f in index.files])]).astype(np.uint32)
+        ptrs = (C.c_void_p * max(n, 1))(*[d.ctypes.data for d in datas])
+        sizes = np.array([d.size for d in datas] or [0], dtype=np.uintp)
+        infos = (_lib.StreamInfoC * max(n, 1))()
+        for i, f in enumerate(index.files):
+            s = f.info
+            infos[i] = _lib.StreamInfoC(s.min_block_size, s.max_block_size, s.min_frame_size or 0, s.max_frame_size or 0,
+                                        s.sample_rate, s.channels, s.bits_per_sample, s.samples or 0,
+                                        (C.c_uint8 * 16)(*s.md5sum))
+        size = int(L.clx_corpus_image_bytes(sizes.ctypes.data, descs.ctypes.data, descs.size, file_frames.ctypes.data, n))
+        if size == 0:
+            raise Error(90, "the index cannot be written as a corpus image")
+        folder, name = os.path.split(os.path.abspath(path))
+        tmp = os.path.join(folder, f".{name}.{os.getpid()}.{secrets.token_hex(4)}.tmp")
+        fd = os.open(tmp, os.O_RDWR | os.O_CREAT | os.O_EXCL, 0o666)
+        mm = None
+        try:
+            os.posix_fallocate(fd, 0, size)
+            mm = mmap.mmap(fd, size, mmap.MAP_SHARED, mmap.PROT_READ | mmap.PROT_WRITE)
+            img = np.frombuffer(mm, dtype=np.uint8)
+            st = L.clx_corpus_image_write(ctx._h, ptrs, sizes.ctypes.data, descs.ctypes.data, descs.size,
+                                          file_frames.ctypes.data, n, infos, img.ctypes.data, size)
+            del img
+            _check(st, ctx)
+            os.link(tmp, path)  # (not rename: a path created meanwhile is refused, never replaced)
+        except BaseException:
+            if mm is not None:
+                mm.close()
+            os.unlink(tmp)
+            raise
+        finally:
+            os.close(fd)
+        os.unlink(tmp)
+        return cls._attach_map(mm, path, ctx)
+
+    @classmethod
+    def attach(cls, source, ctx: Context | None = None) -> "Corpus":
+        """A host corpus over a corpus image (clx_corpus_attach): `source` is the image's path, which is mapped shared
+        and read-write (the driver pins pages writable; the library never writes to them), or an mmap.mmap of one that
+        the caller keeps open for as long as the corpus lives (then several attaches share that one mapping).
+
+        The image is checked in full, its bytes region is registered as pinned memory with cudaHostRegister and only its
+        frame index is copied to the GPU: `device_bytes` is the index alone, and every process and GPU that attaches the
+        image shares the same physical pages.  Crops, packed batches and the bounds work as for Corpus(memory="host"),
+        with the same results.  `memory` is "shared" and `path` the image's path (None for a mapping).  `descs`,
+        `file_frames` and `channels` come from the image, and `index` is a FlacIndex rebuilt from it: each file's
+        StreamInfo, length, frame starts and end_confirmed as written, its `data` a read-only zero-copy view of its
+        bytes in the image (from its first frame to its end), so its descriptors' byte_offset count from there (and
+        out_offset is 0).  close() detaches; the mapping is closed once nothing views it.  The file may be unlinked
+        while attached.  Raises Error(90) for a file that is not a well-formed image."""
+        import mmap
+        import os
+        ctx = ctx or default_context()
+        if isinstance(source, mmap.mmap):
+            return cls._attach_map(source, None, ctx, own=False)
+        path = os.fspath(source)
+        fd = os.open(path, os.O_RDWR)
+        try:
+            size = os.fstat(fd).st_size
+            if size == 0:
+                raise Error(90, f"{path} is empty, not a corpus image")
+            mm = mmap.mmap(fd, size, mmap.MAP_SHARED, mmap.PROT_READ | mmap.PROT_WRITE)
+        finally:
+            os.close(fd)
+        return cls._attach_map(mm, path, ctx)
+
+    @classmethod
+    def _attach_map(cls, mm, path, ctx: Context, own: bool = True) -> "Corpus":
+        self = cls.__new__(cls)
+        self.ctx, self.memory, self.path = ctx, "shared", path
+        img = np.frombuffer(mm, dtype=np.uint8)
+        h = C.c_void_p()
+        st = ctx._L.clx_corpus_attach(ctx._h, img.ctypes.data, img.size, C.byref(h))
+        if st != OK:
+            del img
+            if own:
+                mm.close()
+            _check(st, ctx)
+        self._h, self._map, self._own_map = h, mm, own
+        img.flags.writeable = False
+        hd = _lib.ImageHeader.from_buffer_copy(img[:C.sizeof(_lib.ImageHeader)])
+        recs = (_lib.ImageFile * hd.n_files).from_buffer_copy(img, hd.files_offset)
+        self.descs = np.frombuffer(img, dtype=DESC_DTYPE, count=hd.n_frames, offset=hd.descs_offset).copy()
+        self.file_frames = np.array([r.first_frame for r in recs] + [hd.n_frames], dtype=np.uint32)
+        self.nbytes = int(hd.nbytes)
+        self.channels = max([int(self.descs["n_channels"].max())] if self.descs.size else [1])
+        region = img[hd.bytes_offset:hd.bytes_offset + hd.bytes_size]
+        files = []
+        for i, r in enumerate(recs):
+            d = self.descs[self.file_frames[i]:self.file_frames[i + 1]].copy()
+            d["byte_offset"] -= np.uint64(r.byte_base)
+            files.append(IndexedFile(region[r.byte_base:r.byte_base + r.byte_count], StreamInfo._from_c(r.info), d,
+                                     frame_starts(d), int(d["block_size"].astype(np.int64).sum()),
+                                     bool(r.flags & _lib.IMAGE_END_CONFIRMED)))
+        self.index = FlacIndex(files)
+        return self
+
     def close(self):
-        """Frees the corpus's copy of the bytes and its index; raises Error while a CropBatch of the corpus is alive."""
+        """Frees the corpus's copy of the bytes and its index; raises Error while a CropBatch of the corpus is alive.
+        An attached corpus drops its registration of the image instead, then closes the mapping it opened (at once, or
+        when the last view of it, such as index[i].data, is gone); the image file itself is left as it is."""
         if getattr(self, "_h", None) and getattr(self.ctx, "_h", None):
             _check(self.ctx._L.clx_corpus_destroy(self.ctx._h, self._h), self.ctx)
+            self._h = None
+        if getattr(self, "_h", None) and getattr(self, "_map", None) is not None:
+            _still_registered.append(self._map)  # its context is gone: the pages stay registered, so stay mapped
+            self._own_map = False
         self._h = None
+        if getattr(self, "_own_map", False):
+            self._own_map = False
+            try:
+                self._map.close()
+            except BufferError:  # views of the image are alive: the mapping goes with the last of them
+                pass
 
     def __del__(self):
         try:
             self.close()
         except Exception:
-            pass
+            # Finalized in one garbage cycle with batches of it that are not yet destroyed: the last of them detaches
+            # it (_Batch.close), before the cycle's mapping of the image can be unmapped.
+            self._close_pending = getattr(self, "memory", None) == "shared"
+
+
+# Mappings of images whose corpus could not be detached (its context was closed first): kept mapped for the life of the
+# process, so that no new mapping takes the address range the driver still has registered.
+_still_registered = []
 
 
 class CropBatch:

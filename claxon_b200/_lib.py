@@ -43,7 +43,20 @@ class Options(C.Structure):
                 ("host_threads", C.c_uint32)]
 
 
+class ImageHeader(C.Structure):  # clx_image_header: the header of a corpus image
+    _fields_ = [("magic", C.c_uint64), ("version", C.c_uint32), ("header_bytes", C.c_uint32),
+                ("n_files", C.c_uint64), ("n_frames", C.c_uint64), ("files_offset", C.c_uint64), ("files_bytes", C.c_uint64),
+                ("descs_offset", C.c_uint64), ("descs_bytes", C.c_uint64), ("bytes_offset", C.c_uint64),
+                ("bytes_size", C.c_uint64), ("nbytes", C.c_uint64), ("total_bytes", C.c_uint64)]
+
+
+class ImageFile(C.Structure):  # clx_image_file: one file's record in a corpus image
+    _fields_ = [("info", StreamInfoC), ("byte_base", C.c_uint64), ("byte_count", C.c_uint64),
+                ("first_frame", C.c_uint32), ("n_frames", C.c_uint32), ("flags", C.c_uint32), ("tail", C.c_int32)]
+
+
 assert C.sizeof(FrameDesc) == 40 and C.sizeof(FrameResult) == 8 and C.sizeof(FrameWindow) == 16
+assert C.sizeof(StreamInfoC) == 56 and C.sizeof(ImageHeader) == 96 and C.sizeof(ImageFile) == 88
 
 OPT_NO_VERIFY_CRC = 1
 OPT_GENERIC_KERNEL_ONLY = 2
@@ -54,6 +67,7 @@ OPT_NO_WIDE = 32
 OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT = 1, 2
 BATCH_BYTES_ON_DEVICE = 1
 CORPUS_HOST = 1
+IMAGE_MAGIC, IMAGE_VERSION, IMAGE_ALIGN, IMAGE_END_CONFIRMED = 0x3150524F43584C43, 1, 4096, 1
 OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24 = 0, 1, 2, 3
 OUT_CHANNELS_I32, OUT_CHANNELS_F32 = 4, 5
 FRAME_VARIABLE_BLOCKING = 1
@@ -105,6 +119,10 @@ SYMBOLS = {
     "clx_batch_create_packed": (C.c_int, [_vp, _vp, _sz, _sz, C.c_uint32, C.POINTER(_vp)]),
     "clx_packed_frames_bound": (_sz, [_vp, _sz, _vp, _sz, _sz, _sz]),
     "clx_packed_bytes_bound": (_sz, [_vp, _sz, _vp, _sz, _sz, _sz]),
+    "clx_corpus_image_bytes": (_sz, [_vp, _vp, _sz, _vp, _sz]),
+    "clx_corpus_image_write": (C.c_int, [_vp, _vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz]),
+    "clx_corpus_image_check": (C.c_int, [_vp, _sz]),
+    "clx_corpus_attach": (C.c_int, [_vp, _vp, _sz, C.POINTER(_vp)]),
     "clx_batch_packed_requests": (_vp, [_vp]),
     "clx_batch_packed_count": (_vp, [_vp]),
     "clx_batch_packed_starts": (_vp, [_vp]),

@@ -12,6 +12,7 @@
 #include <chrono>
 #include <condition_variable>
 #include <functional>
+#include <map>
 #include <mutex>
 #include <cstdio>
 #include <cstdlib>
@@ -88,10 +89,12 @@ private:
     bool stop_ = false;
 };
 
-namespace {
 // The size of a device buffer for `nbytes` frame bytes: whole 64-byte TMA chunks + 128 bytes of look-ahead
 // (clx::DecodeBuffers' contract).
-size_t padded_bytes(size_t nbytes) { return ((nbytes + 63) & ~(size_t)63) + 128; }
+size_t clx::padded_bytes(size_t nbytes) { return ((nbytes + 63) & ~(size_t)63) + 128; }
+
+namespace {
+using clx::padded_bytes;
 
 bool is_channels(uint32_t mode) { return mode == CLX_OUT_CHANNELS_I32 || mode == CLX_OUT_CHANNELS_F32; }
 
@@ -237,6 +240,7 @@ struct clx_corpus {
     uint8_t* d_bytes = nullptr; size_t nbytes = 0, buf_bytes = 0;
     uint8_t* h_bytes = nullptr;        // CLX_CORPUS_HOST: the bytes in mapped pinned memory (then d_bytes is null)
     const uint8_t* d_host = nullptr;   // ... and their device address
+    bool attached = false;             // clx_corpus_attach: h_bytes is an image's registered bytes region, buf_bytes long
     size_t device_bytes = 0;           // every device allocation of the corpus
     clx_frame_desc* d_descs = nullptr;  // n_frames + 1: the filler frame last
     int64_t* d_starts = nullptr;
@@ -338,7 +342,13 @@ bool valid_frames(const uint8_t* bytes, size_t nbytes, const clx_frame_desc* des
     }
     return true;
 }
+}  // namespace
 
+bool clx::corpus_frames_ok(const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames) {
+    return valid_frames(bytes, nbytes, descs, n_frames, nullptr);
+}
+
+namespace {
 // Copies per-frame results from the device order to the caller's frame indices: position p holds frame order[p] (an
 // empty order: the same order).
 void unpermute(const clx_frame_result* dev, const std::vector<uint32_t>& order, size_t n, clx_frame_result* results) {
@@ -870,16 +880,84 @@ void clx_host_free(void* p) { if (p) cudaFreeHost(p); }
 // device-resident corpora and crop batches (the kernels: clx_crops.cu)
 // ---------------------------------------------------------------------------------
 namespace {
+// Registrations of corpus images' bytes regions (clx_corpus_attach), process-wide: the same range registered twice is
+// a CUDA error, so contexts that attach one mapping share one registration, counted, and the last detach drops it.
+struct Registry {
+    std::mutex m;
+    std::map<std::pair<const void*, size_t>, int> refs;
+};
+Registry& registry() {
+    static Registry* r = new Registry();  // (never destroyed: a corpus may outlive static destruction order)
+    return *r;
+}
+
+cudaError_t register_range(void* p, size_t n) {
+    Registry& r = registry();
+    std::lock_guard<std::mutex> g(r.m);
+    auto it = r.refs.find({p, n});
+    if (it != r.refs.end()) {
+        it->second++;
+        return cudaSuccess;
+    }
+    const cudaError_t e = cudaHostRegister(p, n, cudaHostRegisterMapped | cudaHostRegisterPortable);
+    if (e == cudaSuccess) r.refs[{p, n}] = 1;
+    else cudaGetLastError();  // (reported here; a later launch check must not see it again)
+    return e;
+}
+
+void unregister_range(void* p, size_t n) {
+    Registry& r = registry();
+    std::lock_guard<std::mutex> g(r.m);
+    auto it = r.refs.find({p, n});
+    if (it == r.refs.end() || --it->second > 0) return;
+    r.refs.erase(it);
+    cudaHostUnregister(p);
+}
+
 void free_corpus(clx_corpus* c) {
     cudaFree(c->d_bytes); cudaFree(c->d_descs); cudaFree(c->d_starts); cudaFree(c->d_file_frames);
     cudaFree(c->d_file_len); cudaFree(c->d_file_ch); cudaFree(c->d_file_tail);
-    if (c->h_bytes) cudaFreeHost(c->h_bytes);
+    if (c->attached) unregister_range(c->h_bytes, c->buf_bytes);
+    else if (c->h_bytes) cudaFreeHost(c->h_bytes);
     delete c;
 }
 
+// Uploads a corpus's frame index: its descriptors (c->descs, the filler frame last), each frame's start, each file's
+// frame range (c->file_frames), length, channel count and trailing-bytes verdict `tail`; sets c->channels / max_bps.
+cudaError_t upload_index(clx_corpus* c, const std::vector<int32_t>& tail) {
+    std::vector<int64_t> starts(c->n_frames), file_len(c->n_files);
+    std::vector<uint32_t> file_ch(c->n_files, 0);
+    for (size_t i = 0; i < c->n_files; i++) {
+        int64_t at = 0;
+        for (size_t f = c->file_frames[i]; f < c->file_frames[i + 1]; f++) {
+            starts[f] = at;
+            at += c->descs[f].block_size;
+            c->channels = std::max<uint32_t>(c->channels, c->descs[f].n_channels);
+            c->max_bps = std::max<uint32_t>(c->max_bps, c->descs[f].bits_per_sample);
+        }
+        file_len[i] = at;
+        if (c->file_frames[i + 1] > c->file_frames[i]) file_ch[i] = c->descs[c->file_frames[i + 1] - 1].n_channels;
+    }
+    cudaError_t e = cudaSuccess;
+    auto put = [&](auto*& dst, const auto& v) {
+        const size_t size = std::max<size_t>(1, v.size()) * sizeof(v[0]);
+        if (e == cudaSuccess) e = cudaMalloc((void**)&dst, size);
+        if (e == cudaSuccess) c->device_bytes += size;
+        if (e == cudaSuccess && !v.empty()) e = cudaMemcpy(dst, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice);
+    };
+    put(c->d_descs, c->descs);
+    put(c->d_starts, starts);
+    put(c->d_file_frames, c->file_frames);
+    put(c->d_file_len, file_len);
+    put(c->d_file_ch, file_ch);
+    put(c->d_file_tail, tail);
+    return e;
+}
+}  // namespace
+
 // The trailing-bytes verdict of a file whose last frame `d` has an unconfirmed end (load()'s check after the last
 // frame): decode the frame; if it decodes and ends before byte_len, the frame header status at its end, unless CLX_EOF.
-int tail_verdict(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, clx_frame_desc d, int32_t* verdict) {
+int clx::tail_verdict(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, clx_frame_desc d, int32_t* verdict) {
     *verdict = CLX_OK;
     d.out_offset = 0;
     std::vector<int32_t> pcm((size_t)d.n_channels * d.block_size);
@@ -894,7 +972,6 @@ int tail_verdict(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, clx_frame_de
     }
     return CLX_OK;
 }
-}  // namespace
 
 extern "C" {
 
@@ -920,34 +997,15 @@ int clx_corpus_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, cons
                 descs[f].byte_offset + descs[f].byte_len < descs[f - 1].byte_offset + descs[f - 1].byte_len)
                 return CLX_ERR_INVALID_ARGUMENT;
     CU(ctx, cudaSetDevice(ctx->device));
-    clx_corpus* c = new clx_corpus();
-    c->n_frames = (uint32_t)n_frames;
-    c->n_files = (uint32_t)n_files;
-    c->nbytes = nbytes;
-    c->file_frames.assign(file_frames, file_frames + n_files + 1);
-    c->descs.assign(descs, descs + n_frames);
-    std::vector<int64_t> starts(n_frames), file_len(n_files);
-    std::vector<uint32_t> file_ch(n_files, 0);
     std::vector<int32_t> tail(n_files, CLX_OK);
     for (size_t i = 0; i < n_files; i++) {
-        int64_t at = 0;
-        for (size_t f = file_frames[i]; f < file_frames[i + 1]; f++) {
-            if (descs[f].n_channels != descs[file_frames[i]].n_channels) {
-                delete c;
-                return CLX_ERR_INVALID_ARGUMENT;
-            }
-            starts[f] = at;
-            at += descs[f].block_size;
-            c->channels = std::max<uint32_t>(c->channels, descs[f].n_channels);
-            c->max_bps = std::max<uint32_t>(c->max_bps, descs[f].bits_per_sample);
-        }
-        file_len[i] = at;
+        for (size_t f = file_frames[i]; f < file_frames[i + 1]; f++)
+            if (descs[f].n_channels != descs[file_frames[i]].n_channels) return CLX_ERR_INVALID_ARGUMENT;
         if (file_frames[i + 1] > file_frames[i]) {
             const clx_frame_desc& last = descs[file_frames[i + 1] - 1];
-            file_ch[i] = last.n_channels;
             if (!(last.flags & CLX_FRAME_CRC16_VERIFIED)) {
-                const int rc = tail_verdict(ctx, bytes, nbytes, last, &tail[i]);
-                if (rc) { delete c; return rc; }
+                const int rc = clx::tail_verdict(ctx, bytes, nbytes, last, &tail[i]);
+                if (rc) return rc;
             }
         }
     }
@@ -955,11 +1013,17 @@ int clx_corpus_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, cons
     const size_t filler_len = clx::filler_frame(filler, sizeof filler);
     clx_frame_desc fd;
     const int fst = clx_parse_frame_header(filler, filler_len, &fd, 0);
-    if (fst != CLX_OK) { delete c; return fst; }
+    if (fst != CLX_OK) return fst;
     fd.byte_offset = nbytes;
     fd.byte_len = (uint32_t)filler_len;
     fd.flags |= CLX_FRAME_CRC16_VERIFIED;
     fd.out_offset = 0;
+    clx_corpus* c = new clx_corpus();
+    c->n_frames = (uint32_t)n_frames;
+    c->n_files = (uint32_t)n_files;
+    c->nbytes = nbytes;
+    c->file_frames.assign(file_frames, file_frames + n_files + 1);
+    c->descs.assign(descs, descs + n_frames);
     c->descs.push_back(fd);
     c->buf_bytes = padded_bytes(nbytes + filler_len);
     cudaError_t e = cudaSuccess;
@@ -978,21 +1042,38 @@ int clx_corpus_create_ex(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, cons
         if (e == cudaSuccess && nbytes) e = cudaMemcpy(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice);
         if (e == cudaSuccess) e = cudaMemcpy(c->d_bytes + nbytes, filler, filler_len, cudaMemcpyHostToDevice);
     }
-    auto put = [&](auto*& dst, const auto& v) {
-        const size_t size = std::max<size_t>(1, v.size()) * sizeof(v[0]);
-        if (e == cudaSuccess) e = cudaMalloc((void**)&dst, size);
-        if (e == cudaSuccess) c->device_bytes += size;
-        if (e == cudaSuccess && !v.empty()) e = cudaMemcpy(dst, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice);
-    };
-    put(c->d_descs, c->descs);
-    put(c->d_starts, starts);
-    put(c->d_file_frames, c->file_frames);
-    put(c->d_file_len, file_len);
-    put(c->d_file_ch, file_ch);
-    put(c->d_file_tail, tail);
+    if (e == cudaSuccess) e = upload_index(c, tail);
     if (e != cudaSuccess) {
         free_corpus(c);
         return cuda_fail(ctx, e, "clx_corpus_create");
+    }
+    *out = c;
+    return CLX_OK;
+}
+
+int clx_corpus_attach(clx_ctx* ctx, void* image, size_t image_bytes, clx_corpus** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    clx::ImageIndex ix;
+    if (!ctx || clx::read_image(image, image_bytes, &ix) != CLX_OK) return CLX_ERR_INVALID_ARGUMENT;
+    CU(ctx, cudaSetDevice(ctx->device));
+    uint8_t* region = static_cast<uint8_t*>(image) + ix.bytes_offset;
+    cudaError_t e = register_range(region, ix.bytes_size);
+    if (e != cudaSuccess) return cuda_fail(ctx, e, "clx_corpus_attach: cudaHostRegister");
+    clx_corpus* c = new clx_corpus();
+    c->attached = true;  // from here on free_corpus drops the registration
+    c->h_bytes = region;
+    c->buf_bytes = ix.bytes_size;
+    c->nbytes = ix.nbytes;
+    c->n_files = (uint32_t)ix.tail.size();
+    c->n_frames = (uint32_t)ix.descs.size() - 1;
+    c->descs = std::move(ix.descs);
+    c->file_frames = std::move(ix.file_frames);
+    e = cudaHostGetDevicePointer((void**)&c->d_host, region, 0);
+    if (e == cudaSuccess) e = upload_index(c, ix.tail);
+    if (e != cudaSuccess) {
+        free_corpus(c);
+        return cuda_fail(ctx, e, "clx_corpus_attach");
     }
     *out = c;
     return CLX_OK;

@@ -3,6 +3,7 @@
 #define CLX_INTERNAL_H
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <vector>
 #include "claxon_b200.h"
 
 // Device-only marker: the frame has an LPC order above what the first kernel instance keeps in
@@ -144,6 +145,22 @@ struct PackedBuffers {
 };
 // Filler frame: 1 channel, 16 bits, block size 192, CONSTANT 0.  Writes it if cap suffices; returns its length.
 size_t filler_frame(uint8_t* out, size_t cap);
+// clx_api.cu, for corpus images (clx_corpus_image.cpp): the size of a frame-bytes buffer of `nbytes` bytes (whole
+// 64-byte chunks + 128 bytes of look-ahead); the per-frame checks of clx_corpus_create_ex (byte range and the shapes the
+// kernels decode); the trailing-bytes verdict of a file whose last frame `d` has an unconfirmed end.
+size_t padded_bytes(size_t nbytes);
+bool corpus_frames_ok(const uint8_t* bytes, size_t nbytes, const clx_frame_desc* descs, size_t n_frames);
+int tail_verdict(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, clx_frame_desc d, int32_t* verdict);
+// clx_corpus_image.cpp: what clx_corpus_attach takes from an image that clx_corpus_image_check accepted, copied out of
+// it.  descs: n_frames + 1, the filler frame last, byte_offset into the bytes region; file_frames: n_files + 1.
+struct ImageIndex {
+    uint64_t bytes_offset = 0, bytes_size = 0, nbytes = 0;
+    std::vector<clx_frame_desc> descs;
+    std::vector<uint32_t> file_frames;
+    std::vector<int32_t> tail;
+};
+// CLX_OK with `ix` filled, or CLX_ERR_INVALID_ARGUMENT (clx_corpus_image_check's verdict).
+int read_image(const void* image, size_t image_bytes, ImageIndex* ix);
 // The crop batch's launch sequence: planner (count, scan, the gather of a host corpus, emit, zero-fill), launch_decode
 // over every slot, status pass.  `db`: the batch's buffers; db.descs / db.cols / db.wins are written by the planner, and
 // over a host corpus db.bytes is the staging buffer the gather writes.

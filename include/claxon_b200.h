@@ -386,6 +386,77 @@ size_t clx_packed_frames_bound(const clx_frame_desc* descs, size_t n_frames, con
  * 16 per excerpt for alignment.  SIZE_MAX if that overflows.  Host only.  0 for a bad file_frames or a zero argument. */
 size_t clx_packed_bytes_bound(const clx_frame_desc* descs, size_t n_frames, const uint32_t* file_frames, size_t n_files,
                               size_t max_excerpts, size_t max_samples);
+/* Shared host corpora: a corpus IMAGE is one file, written once (normally on a tmpfs such as /dev/shm), that holds a
+ * host corpus's frame index and bytes; every process and GPU of a machine maps it and attaches it, so the pinned bytes
+ * exist once per machine instead of once per context.  All integers little-endian, at these offsets:
+ *   [0, 96)                           clx_image_header
+ *   [files_offset, + files_bytes)     clx_image_file (88 bytes) per file; files_offset = 128
+ *   [descs_offset, + (n_frames+1)*40) clx_frame_desc: the corpus's frames, file by file in stream order, byte_offset
+ *                                     relative to the bytes region and out_offset 0, then the filler frame of
+ *                                     clx_crop_filler_frame (byte_offset nbytes, its exact byte_len, flags
+ *                                     CLX_FRAME_CRC16_VERIFIED); descs_offset = files_offset + files_bytes rounded up
+ *                                     to 64
+ *   [bytes_offset, + bytes_size)      the bytes region, as a host corpus holds it: each file's bytes from its first frame
+ *                                     to its end, back to back (nbytes in all), the filler frame, zeros up to
+ *                                     bytes_size = round_up_64(nbytes + filler length) + 128; bytes_offset =
+ *                                     descs_offset + descs_bytes rounded up to CLX_IMAGE_ALIGN
+ * total_bytes = bytes_offset + bytes_size, and every gap between sections is zero.  Only the bytes region is read
+ * after attaching; the header, file records and descriptors are copied (validated) once.
+ *
+ * clx_corpus_image_bytes: the size of the image of n_files files, file i being file_nbytes[i] bytes whose frames are
+ * descs[file_frames[i] .. file_frames[i + 1]) with byte_offset into that file; 0 for a bad file_frames, a first frame
+ * past its file's end, or a size that overflows.  Host only.
+ * clx_corpus_image_write: writes that image into image[0, image_bytes), image_bytes being exactly that size, copying
+ * file i's bytes straight from file_bytes[i] (e.g. its memory map) and infos[i] into its record.  It refuses
+ * (CLX_ERR_INVALID_ARGUMENT) what clx_corpus_create_ex(..., CLX_CORPUS_HOST) refuses, each file's frames checked
+ * against its own buffer, and a file_frames[0] other than 0 (frames outside every file); it computes each file's trailing-bytes verdict once, as clx_corpus_create_ex does (a file
+ * whose last frame lacks CLX_FRAME_CRC16_VERIFIED has that frame decoded on the context's device).  The magic is
+ * stored last, so an image whose magic reads right was written through.
+ * clx_corpus_image_check: CLX_OK if image[0, image_bytes) is a well-formed image, else CLX_ERR_INVALID_ARGUMENT: the
+ * magic, version, header size, counts (below 2^32 - 1), every offset and size against the layout above, image_bytes ==
+ * total_bytes, the gaps and padding zero, the filler frame and its descriptor, each frame as the create calls check it
+ * and inside its file's bytes, each file's frames in byte order with one channel count, starting at its byte_base, the
+ * files' bytes and frame ranges back to back, flags and verdicts as the writer sets them.  Host only; no context.
+ * clx_corpus_attach: checks the image, registers its bytes region with cudaHostRegister (mapped, portable), uploads the
+ * frame index, and returns a host corpus over those pages: crop and packed batches, clx_corpus_device_bytes (the index
+ * only) and clx_corpus_destroy work on it as on any CLX_CORPUS_HOST corpus, with the same results.  The registration is
+ * counted in a process-wide registry keyed by address and length, so contexts of one process, on one device or on
+ * several, can attach the same mapping; the last destroy unregisters it (destroy never frees the image, which belongs to
+ * the caller and must stay mapped until then).  A refused or failed attach leaves nothing registered.  The mapping must
+ * be writable (the driver pins pages writable); the library never writes to it.  If the bytes region changes after
+ * attaching, the crops that read the changed bytes get wrong samples or a CRC error, never an access outside the
+ * region: every span comes from the index copied at attach time. */
+#define CLX_IMAGE_MAGIC 0x3150524f43584c43ull /* the bytes "CLXCORP1" */
+#define CLX_IMAGE_VERSION 1u
+#define CLX_IMAGE_ALIGN 4096u
+#define CLX_IMAGE_END_CONFIRMED 1u /* clx_image_file.flags: the file has no frames, or its last frame's end is confirmed */
+typedef struct clx_image_header {
+    uint64_t magic;          /* CLX_IMAGE_MAGIC */
+    uint32_t version;        /* CLX_IMAGE_VERSION */
+    uint32_t header_bytes;   /* sizeof(clx_image_header) = 96 */
+    uint64_t n_files, n_frames;
+    uint64_t files_offset, files_bytes;  /* n_files * sizeof(clx_image_file) */
+    uint64_t descs_offset, descs_bytes;  /* (n_frames + 1) * sizeof(clx_frame_desc) */
+    uint64_t bytes_offset, bytes_size;
+    uint64_t nbytes;         /* the files' bytes at the start of the region */
+    uint64_t total_bytes;
+} clx_image_header;
+typedef struct clx_image_file {
+    clx_streaminfo info;     /* as given to the writer */
+    uint64_t byte_base;      /* where the file's bytes start in the region: the sum of the byte_counts before it */
+    uint64_t byte_count;     /* its bytes from its first frame to its end; 0 for a file without frames */
+    uint32_t first_frame;    /* its frames are descriptors [first_frame, first_frame + n_frames) */
+    uint32_t n_frames;
+    uint32_t flags;          /* CLX_IMAGE_END_CONFIRMED or 0 */
+    int32_t tail;            /* trailing-bytes verdict: CLX_OK, or a frame header status 2..10 when the end is unconfirmed */
+} clx_image_file;
+size_t clx_corpus_image_bytes(const size_t* file_nbytes, const clx_frame_desc* descs, size_t n_frames,
+                              const uint32_t* file_frames, size_t n_files);
+int clx_corpus_image_write(clx_ctx* ctx, const uint8_t* const* file_bytes, const size_t* file_nbytes,
+                           const clx_frame_desc* descs, size_t n_frames, const uint32_t* file_frames, size_t n_files,
+                           const clx_streaminfo* infos, void* image, size_t image_bytes);
+int clx_corpus_image_check(const void* image, size_t image_bytes);
+int clx_corpus_attach(clx_ctx* ctx, void* image, size_t image_bytes, clx_corpus** out);
 /* Device pointers of a packed batch (NULL for other batches): max_excerpts requests (zeroed at creation); one uint32, how
  * many of them a call uses (0 at creation); max_excerpts int64 column starts, written by each call.  The row stride of
  * the output in elements (0 for other batches). */

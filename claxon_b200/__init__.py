@@ -14,6 +14,7 @@ plumbing.  Nothing here imports the test oracle.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass
 
 import numpy as np
@@ -1022,11 +1023,19 @@ class Corpus:
         return int(self.ctx._L.clx_crop_bytes_bound(self.descs.ctypes.data, self.descs.size, self.file_frames.ctypes.data,
                                                     len(self.index), int(num_frames)))
 
-    def crops(self, batch: int, num_frames: int, dtype=None) -> "CropBatch":
+    def crops(self, batch: int, num_frames: int, dtype=None, sample_rate: int | None = None) -> "CropBatch":
         """A CropBatch of `batch` crops of `num_frames` samples; its CUDA graph is instantiated here.  Over a host
         corpus, the batch also holds a GPU staging buffer of about batch x bytes_bound(num_frames) bytes, and each call
-        reads the selected crops' span bytes (about span bytes x batch) from host memory over PCIe."""
-        return CropBatch(self, batch, num_frames, dtype)
+        reads the selected crops' span bytes (about span bytes x batch) from host memory over PCIe.  With `sample_rate`
+        R, every crop is at rate R whatever its file's rate: offsets and num_frames count samples at R (see CropBatch)."""
+        return CropBatch(self, batch, num_frames, dtype, sample_rate)
+
+    def resample_source_bound(self, num_frames: int, sample_rate: int) -> int:
+        """The most source samples a crop of num_frames samples at `sample_rate` reads from one file of the corpus
+        (clx_resample_source_bound, the largest over the files' rates)."""
+        L = self.ctx._L
+        return max([int(L.clx_resample_source_bound(f.info.sample_rate, int(sample_rate), int(num_frames)))
+                    for f in self.index.files] or [0])
 
     def packed_frames_bound(self, max_excerpts: int, max_samples: int) -> int:
         """clx_packed_frames_bound: the most frames the excerpts of one packed call can overlap together."""
@@ -1223,19 +1232,39 @@ class CropBatch:
 
     Over a host corpus (Corpus(memory="host")), each call first copies every crop's span of frames from pinned host
     memory into a GPU staging buffer, one more kernel in the graph: about span bytes x B cross PCIe per call.  Results
-    are the same as over a device corpus."""
+    are the same as over a device corpus.
 
-    def __init__(self, corpus: Corpus, batch: int, num_frames: int, dtype=None):
+    With `sample_rate` R (clx_batch_create_resampled_crops; float32 only), files of any rate give crops at rate R:
+    offsets and L count samples at R, and crop b is resample(x, r, R)[:, offsets[b] : offsets[b] + L], x the whole file
+    as load() gives it and r its STREAMINFO rate, resample being torchaudio.functional.resample with its defaults (so
+    the samples near a crop's edges are those of the resampled file, not of a resampled excerpt).  lengths[b] =
+    min(L, N_t - offsets[b]) with N_t = ceil(N * R / r) the file's length at R; an offset past N_t is invalid.  Files
+    already at R are copied, bit for bit what a batch without sample_rate gives.  A crop's status is that of its source
+    span, the samples its outputs read.  Each call decodes every crop's source span with a packed batch of
+    B x round_up_4(resample_source_bound(L, R)) columns (about L x r / R samples per crop and row) and filters them on
+    the device."""
+
+    def __init__(self, corpus: Corpus, batch: int, num_frames: int, dtype=None, sample_rate: int | None = None):
         import torch
         dtype = _torch_dtype(dtype)
         self.corpus, self.ctx = corpus, corpus.ctx
         self.batch, self.num_frames, self.dtype = int(batch), int(num_frames), dtype
+        self.sample_rate = None if sample_rate is None else int(sample_rate)
         if self.batch < 1 or self.num_frames < 1:
             raise ValueError("batch and num_frames must be >= 1")
         mode = _channels_mode(dtype)
         L = self.ctx._L
         h = C.c_void_p()
-        _check(L.clx_batch_create_crops(self.ctx._h, corpus._h, self.batch, self.num_frames, mode, C.byref(h)), self.ctx)
+        if self.sample_rate is None:
+            _check(L.clx_batch_create_crops(self.ctx._h, corpus._h, self.batch, self.num_frames, mode, C.byref(h)),
+                   self.ctx)
+        else:
+            if dtype != torch.float32:
+                raise ValueError("a resampled crop batch is float32 only")
+            rates = np.array([f.info.sample_rate for f in corpus.index.files] or [0], dtype=np.uint32)
+            _check(L.clx_batch_create_resampled_crops(self.ctx._h, corpus._h, rates.ctypes.data, len(corpus.index),
+                                                      self.batch, self.num_frames, self.sample_rate, C.byref(h)),
+                   self.ctx)
         self._batch = _Batch(self.ctx, h, keep=corpus)
         self.channels = corpus.channels
         B, view = self.batch, self._batch.tensor
@@ -1291,7 +1320,12 @@ class CropBatch:
         if kind == 0:
             if not 0 <= fi < len(self.corpus.index):
                 raise ValueError(f"crop {b}: file index {fi} out of range")
-            raise ValueError(f"crop {b}: offset {o} outside file {fi} ({self.corpus.index[fi].length} samples)")
+            f = self.corpus.index[fi]
+            if self.sample_rate is None or f.info.sample_rate == self.sample_rate:
+                raise ValueError(f"crop {b}: offset {o} outside file {fi} ({f.length} samples)")
+            g = math.gcd(f.info.sample_rate, self.sample_rate)
+            Nt = -(-f.length * (self.sample_rate // g) // (f.info.sample_rate // g))
+            raise ValueError(f"crop {b}: offset {o} outside file {fi} ({Nt} samples at {self.sample_rate} Hz)")
         raise Error(st, f"file {fi}, crop {b}")
 
     def kernel_ms(self) -> float:

@@ -234,6 +234,11 @@ struct clx_batch {
     uint64_t span_stride = 0;
     bool is_packed = false;
     clx::PackedBuffers packed{};
+    // Resampled crop batches (clx_batch_create_resampled_crops): crop batches whose graph runs `inner`, a packed batch,
+    // between the map and filter kernels.  crop.requests and crop.lengths are their own, crop.status and crop.error
+    // the inner batch's; buf.conv is the output; rs the rest.
+    clx_batch* inner = nullptr;
+    clx::ResampleBuffers rs{};
 };
 
 struct clx_corpus {
@@ -679,6 +684,13 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
 
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
     const clx::DecodeBuffers db = b->buf.view(b->n_frames, b->mode, b->stride);
+    if (b->inner) {
+        const clx::CropCorpus cc = b->corpus->view(0);
+        cudaError_t e = clx::launch_resample_map(cc, b->rs, st, launches);
+        if (e == cudaSuccess) e = launch_batch(b->inner, st, launches);
+        if (e == cudaSuccess) e = clx::launch_resample(b->rs, st, launches);
+        return e;
+    }
     if (b->corpus && b->is_packed)
         return clx::launch_packed(b->corpus->view(b->span_stride), b->crop, b->packed, db, b->plan, b->device_crc, st,
                                   launches);
@@ -693,7 +705,7 @@ void build_graph(clx_ctx* ctx, clx_batch* b) {
 #ifdef CLX_EXPERIMENT
     if (getenv("CLX_NO_GRAPH")) return;
 #endif
-    if (b->n_frames == 0) return;
+    if (b->n_frames == 0 && !b->inner) return;
     cudaStream_t st = ctx->streams[0];
     cudaGraph_t g = nullptr;
     uint64_t n = 0;
@@ -807,6 +819,13 @@ void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
     (void)ctx;
     if (!b) return;
     b->buf.release();
+    if (b->inner) {
+        b->crop.status = nullptr;  // the inner batch's
+        b->crop.error = nullptr;
+        cudaFree(b->rs.plan); cudaFree((void*)b->rs.file_rate); cudaFree((void*)b->rs.rates); cudaFree((void*)b->rs.coefs);
+        cudaFree((void*)b->rs.k0);
+        clx_batch_destroy(ctx, b->inner);
+    }
     if (b->corpus) {
         b->corpus->live--;
         cudaFree((void*)b->crop.requests); cudaFree(b->crop.status); cudaFree(b->crop.lengths); cudaFree(b->crop.error);
@@ -1104,6 +1123,15 @@ cudaError_t device_zeros(const T*& p, size_t n) {
     p = q;
     return e;
 }
+// A device copy of a host table (one element at least, so that an empty table is a valid pointer too).
+template <typename T>
+cudaError_t upload(const T*& p, const std::vector<T>& v) {
+    T* q = nullptr;
+    cudaError_t e = cudaMalloc((void**)&q, std::max<size_t>(v.size(), 1) * sizeof(T));
+    p = q;
+    if (e == cudaSuccess && !v.empty()) e = cudaMemcpy(q, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
+    return e;
+}
 
 // The per-excerpt buffers every crop or packed batch's planner writes (all but the requests), and its timing events.
 cudaError_t alloc_planner(clx_batch* b, size_t n) {
@@ -1263,6 +1291,70 @@ void* clx_batch_packed_requests(clx_batch* b) { return b && b->is_packed ? (void
 void* clx_batch_packed_count(clx_batch* b) { return b && b->is_packed ? (void*)b->packed.count : nullptr; }
 void* clx_batch_packed_starts(clx_batch* b) { return b && b->is_packed ? (void*)b->packed.starts : nullptr; }
 size_t clx_batch_packed_stride(clx_batch* b) { return b && b->is_packed ? b->stride : 0; }
+
+int clx_batch_create_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                                     size_t n_crops, size_t num_frames, uint32_t target_rate, clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (!ctx || !corpus || !file_rates || n_files != corpus->n_files || n_crops == 0 || num_frames == 0 ||
+        n_crops >= (1u << 30))
+        return CLX_ERR_INVALID_ARGUMENT;
+    clx::ResampleTables t;
+    if (!clx::resample_tables(file_rates, n_files, target_rate, num_frames, &t)) return CLX_ERR_INVALID_ARGUMENT;
+    // The inner packed batch: every crop's source span fits in its round_up_4(bound) columns.
+    const size_t C = corpus->channels, rows = n_crops * C;  // (< 2^33: no overflow)
+    if (t.bound > (SIZE_MAX / 16) / n_crops || num_frames > (SIZE_MAX / 4 - 8) / rows ||
+        (num_frames + t.tile - 1) / t.tile >= (1u << 31))
+        return CLX_ERR_INVALID_ARGUMENT;
+    clx_batch* inner = nullptr;
+    const int rc = clx_batch_create_packed(ctx, corpus, n_crops, n_crops * ((t.bound + 3) & ~(size_t)3),
+                                           CLX_OUT_CHANNELS_F32, &inner);
+    if (rc != CLX_OK) return rc;
+    clx_batch* b = new clx_batch();
+    b->corpus = corpus;
+    corpus->live++;
+    b->inner = inner;
+    b->out_elems = rows * num_frames;
+    b->mode = CLX_OUT_CHANNELS_F32;
+    b->stride = num_frames;
+    clx::CropBuffers& cb = b->crop;
+    cb.n_crops = (uint32_t)n_crops;
+    cb.C = (uint32_t)C;
+    cb.L = num_frames;
+    cb.status = inner->crop.status;
+    cb.error = inner->crop.error;
+    clx::ResampleBuffers& rs = b->rs;
+    rs.n_crops = (uint32_t)n_crops;
+    rs.C = (uint32_t)C;
+    rs.L = num_frames;
+    rs.tile = t.tile;
+    rs.excerpts = const_cast<clx_packed_request*>(inner->packed.requests);
+    rs.count = const_cast<uint32_t*>(inner->packed.count);
+    rs.starts = inner->packed.starts;
+    rs.src = static_cast<const float*>((const void*)inner->buf.conv);
+    rs.src_stride = inner->stride;
+    cudaError_t e = cudaSetDevice(ctx->device);
+    if (e == cudaSuccess) e = device_zeros(cb.requests, n_crops);
+    if (e == cudaSuccess) e = device_zeros(cb.lengths, n_crops);
+    if (e == cudaSuccess) e = device_zeros(b->buf.conv, (b->out_elems + 8) * sizeof(float));  // (the slack of fit())
+    if (e == cudaSuccess) e = cudaMalloc((void**)&rs.plan, n_crops * sizeof(clx::ResamplePlan));
+    if (e == cudaSuccess) e = upload(rs.file_rate, t.file_rate);
+    if (e == cudaSuccess) e = upload(rs.rates, t.rates);
+    if (e == cudaSuccess) e = upload(rs.coefs, t.coefs);
+    if (e == cudaSuccess) e = upload(rs.k0, t.k0);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
+    if (e != cudaSuccess) {
+        clx_batch_destroy(ctx, b);
+        return cuda_fail(ctx, e, "clx_batch_create_resampled_crops");
+    }
+    rs.requests = cb.requests;
+    rs.lengths = cb.lengths;
+    rs.out = reinterpret_cast<float*>(b->buf.conv);
+    build_graph(ctx, b);
+    *out = b;
+    return CLX_OK;
+}
 
 }  // extern "C"
 

@@ -169,6 +169,54 @@ cudaError_t launch_crops(const CropCorpus& cc, const CropBuffers& cb, const Deco
 // The packed batch's launch sequence, of the same shape (clx_crops.cu).
 cudaError_t launch_packed(const CropCorpus& cc, const CropBuffers& cb, const PackedBuffers& pb, const DecodeBuffers& db,
                           const Plan& plan, bool crc, cudaStream_t stream, uint64_t* launches);
+
+// clx_resample.cu: resampled crop batches (clx_batch_create_resampled_crops), a packed batch of each crop's source span
+// between two kernels.  One polyphase table per distinct source rate r != R: with g = gcd(r, R), o = r / g, n = R / g,
+// output blk * n + ph is sum_i coef[i * n + ph] * x[blk * o + k0[ph] + i]; taps 0 marks r == R (copied).
+struct ResampleRate {
+    uint32_t o, n, w, taps;
+    uint64_t coef;  // the table's first coefficient in ResampleBuffers::coefs
+    uint64_t k0;    // its first k0 in ResampleBuffers::k0 (n of them, each in [-w, w + o - taps])
+};
+// Per crop, what resample_map_kernel found (device memory, written every decode).
+struct ResamplePlan {
+    int64_t offset;            // first output sample, at rate R
+    int64_t src_lo, src_len;   // the source span decoded for it: samples [src_lo, src_lo + src_len) of its file
+    uint32_t rate;             // its file's ResampleRate
+    uint32_t ch;               // rows the crop covers (0: an invalid request)
+};
+struct ResampleBuffers {
+    const clx_crop_request* requests;
+    int64_t* lengths;               // at rate R
+    ResamplePlan* plan;
+    const uint32_t* file_rate;      // per file, its ResampleRate
+    const ResampleRate* rates;
+    const float* coefs;
+    const int32_t* k0;
+    clx_packed_request* excerpts;   // the inner packed batch's requests and count, written by the map kernel
+    uint32_t* count;
+    const int64_t* starts;          // ... its column starts
+    const float* src;               // ... and output, rows of src_stride
+    uint64_t src_stride;
+    float* out;                     // [n_crops * C, L]
+    uint32_t n_crops, C, tile;      // tile: outputs per CTA of resample_kernel
+    uint64_t L;
+};
+// The host side of clx_batch_create_resampled_crops: the tables of the distinct rates of file_rates towards target, and
+// the longest source span of a crop (clx_resample_source_bound over those rates).  false for a rate of 0 or above
+// CLX_MAX_SAMPLE_RATE, or more than 2^24 coefficients in all.
+struct ResampleTables {
+    std::vector<ResampleRate> rates;
+    std::vector<uint32_t> file_rate;
+    std::vector<float> coefs;
+    std::vector<int32_t> k0;
+    uint64_t bound = 0;
+    uint32_t tile = 0;
+};
+bool resample_tables(const uint32_t* file_rates, size_t n_files, uint32_t target, size_t num_frames, ResampleTables* t);
+// The two kernels around the packed batch's launch sequence.
+cudaError_t launch_resample_map(const CropCorpus& cc, const ResampleBuffers& rs, cudaStream_t stream, uint64_t* launches);
+cudaError_t launch_resample(const ResampleBuffers& rs, cudaStream_t stream, uint64_t* launches);
 #ifdef CLX_EXPERIMENT
 extern int g_exp_which;  // measurement builds only: bit 0 = index pass, bit 1 = decode pass of LanePerFrame
 extern int g_exp_dyn_smem;

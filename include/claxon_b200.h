@@ -464,6 +464,34 @@ void* clx_batch_packed_requests(clx_batch* b);
 void* clx_batch_packed_count(clx_batch* b);
 void* clx_batch_packed_starts(clx_batch* b);
 size_t clx_batch_packed_stride(clx_batch* b);
+/* Resampled crop batches: crop batches of a corpus whose files may have different sample rates, every crop at one
+ * target rate R.  file_rates[i] is file i's rate r_i (its STREAMINFO sample_rate); n_files must be the corpus's.  Crop b
+ * of request {file, 0, offset} is resample(x, r, R)[:, offset : offset + num_frames], x the whole file, where resample is
+ * torchaudio.functional.resample with its defaults (lowpass_filter_width 6, rolloff 0.99, sinc_interp_hann): with g =
+ * gcd(r, R), o = r / g, n = R / g, base = min(o, n) * 0.99 and w = ceil(6 * o / base), output j = blk * n + ph is
+ * sum h[ph, k] * x[blk * o + k] over k in [-w, w + o), samples outside the file reading 0, h = sinc(t) * cos(t * pi /
+ * 12)^2 * base / o with t = (k / o - ph / n) * base (taps with |t| >= 6 are skipped); N_t = ceil(N * n / o) outputs.
+ * A file with r == R is copied, not filtered (N_t = N), bit for bit what clx_batch_create_crops gives.
+ * The output is [n_crops * C, num_frames] float32 (CLX_OUT_CHANNELS_F32), C the corpus's largest channel count.  The
+ * crop accessors serve the batch: requests (clx_crop_request, offsets at rate R), status, lengths (min(num_frames, N_t -
+ * offset), 0 for an invalid request), error and clx_batch_device_out.  A request with file >= n_files, reserved != 0,
+ * offset < 0 or > N_t is invalid (status CLX_ERR_INVALID_ARGUMENT, kind 0 in the error word, zero rows); a valid crop's
+ * status and error word are those of a crop of its source span: the samples its outputs read, clipped to the file.
+ * Columns past a crop's length and rows its file does not have read 0.
+ * Each call decodes every crop's source span with the launch sequence of a packed batch, sized so that every span fits
+ * (n_crops columns of round_up_4 of the largest clx_resample_source_bound over the corpus's rates), between a kernel
+ * that maps the requests to source spans and the filter kernel, which writes every element of the output.
+ * CLX_ERR_INVALID_ARGUMENT for: a rate or target rate of 0 or above CLX_MAX_SAMPLE_RATE, more than 2^24 filter
+ * coefficients over the distinct rates (n times the taps per phase each), what clx_batch_create_packed refuses for that
+ * size in CLX_OUT_CHANNELS_F32 (frames above 24 bits among them), n_crops 0 or 2^30 or more, num_frames 0, sizes that
+ * overflow. */
+#define CLX_MAX_SAMPLE_RATE 655350u
+int clx_batch_create_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                                     size_t n_crops, size_t num_frames, uint32_t target_rate, clx_batch** out);
+/* The most source samples a resampled crop of num_frames outputs reads from a file of rate orig: num_frames when orig ==
+ * target, else (floor((num_frames - 1) / n) + 2) * o + 2w.  SIZE_MAX if that overflows; 0 for a zero argument or a rate
+ * above CLX_MAX_SAMPLE_RATE.  Host only. */
+size_t clx_resample_source_bound(uint32_t orig, uint32_t target, size_t num_frames);
 int clx_batch_decode(clx_ctx* ctx, clx_batch* b, uint32_t stream_index); /* async on an internal stream */
 int clx_batch_sync(clx_ctx* ctx, clx_batch* b);
 /* Planar batches only (CLX_ERR_INVALID_ARGUMENT for any other mode). */

@@ -1047,10 +1047,18 @@ class Corpus:
         return int(self.ctx._L.clx_packed_bytes_bound(self.descs.ctypes.data, self.descs.size, self.file_frames.ctypes.data,
                                                       len(self.index), int(max_excerpts), int(max_samples)))
 
-    def packed(self, max_excerpts: int, max_samples: int, dtype=None) -> "PackedBatch":
+    def packed(self, max_excerpts: int, max_samples: int, dtype=None, sample_rate: int | None = None) -> "PackedBatch":
         """A PackedBatch of up to `max_excerpts` excerpts laid out along `max_samples` columns; its CUDA graph is
-        instantiated here."""
-        return PackedBatch(self, max_excerpts, max_samples, dtype)
+        instantiated here.  With `sample_rate` R, every excerpt is at rate R whatever its file's rate: offsets, lengths,
+        max_samples and the starts count samples at R (see PackedBatch)."""
+        return PackedBatch(self, max_excerpts, max_samples, dtype, sample_rate)
+
+    def resample_packed_source_bound(self, max_excerpts: int, max_samples: int, sample_rate: int) -> int:
+        """clx_resample_packed_source_bound: the columns of the packed batch that decodes the source spans of a
+        resampled PackedBatch (about max_samples x r / R for the corpus's highest rate r)."""
+        rates = np.array([f.info.sample_rate for f in self.index.files] or [0], dtype=np.uint32)
+        return int(self.ctx._L.clx_resample_packed_source_bound(rates.ctypes.data, len(self.index), int(sample_rate),
+                                                                int(max_excerpts), int(max_samples)))
 
     @classmethod
     def share(cls, index: FlacIndex, path, ctx: Context | None = None) -> "Corpus":
@@ -1364,20 +1372,41 @@ class PackedBatch:
     stream has enqueued before it.  A float32 batch is refused when any frame of the corpus has more than 24 bits.
     Memory: C x (T + the trash columns) output elements and a planar scratch of the corpus's largest frame for each of
     packed_frames_bound(max_excerpts, T) slots; over a host corpus also a staging buffer of packed_bytes_bound() bytes,
-    and each call reads the selected spans over PCIe."""
+    and each call reads the selected spans over PCIe.
 
-    def __init__(self, corpus: Corpus, max_excerpts: int, max_samples: int, dtype=None):
+    With `sample_rate` R (clx_batch_create_resampled_packed; float32 only), files of any rate give excerpts at rate R,
+    with the filter of CropBatch's `sample_rate`.  Everything counts samples at R: offsets, lengths, T, the starts and
+    the returned lengths.  Excerpt b is resample(x, r, R)[:, offsets[b] : offsets[b] + n_b], x the whole file as load()
+    gives it and r its STREAMINFO rate, with n_b = min(lengths[b], N_t - offsets[b]) and N_t = ceil(N * R / r) the
+    file's length at R; so the samples near an excerpt's edges are those of the resampled file, not zero-padded.  An
+    offset past N_t is invalid, one at N_t the valid empty excerpt; the layout and the fit rule are those above.  Files
+    already at R are copied: over a corpus whose files are all at R, a call gives what a float32 batch without
+    sample_rate gives, bit for bit.  An excerpt's status is that of its source span, the samples its outputs read.
+    Memory: the [C, round_up_4(T)] output, and an inner packed batch of T_src = resample_packed_source_bound(max_excerpts,
+    T, R) columns that decodes every excerpt's source span (about C x T_src float32 plus its slot scratch, so about T x
+    r / R samples per row for the highest rate r: 6 x T for 96 kHz to 16 kHz)."""
+
+    def __init__(self, corpus: Corpus, max_excerpts: int, max_samples: int, dtype=None, sample_rate: int | None = None):
         import torch
         dtype = _torch_dtype(dtype)
         self.corpus, self.ctx = corpus, corpus.ctx
         self.max_excerpts, self.max_samples, self.dtype = int(max_excerpts), int(max_samples), dtype
+        self.sample_rate = None if sample_rate is None else int(sample_rate)
         if self.max_excerpts < 1 or self.max_samples < 1:
             raise ValueError("max_excerpts and max_samples must be >= 1")
         mode = _channels_mode(dtype)
         L = self.ctx._L
         h = C.c_void_p()
-        _check(L.clx_batch_create_packed(self.ctx._h, corpus._h, self.max_excerpts, self.max_samples, mode, C.byref(h)),
-               self.ctx)
+        if self.sample_rate is None:
+            _check(L.clx_batch_create_packed(self.ctx._h, corpus._h, self.max_excerpts, self.max_samples, mode,
+                                             C.byref(h)), self.ctx)
+        else:
+            if dtype != torch.float32:
+                raise ValueError("a resampled packed batch is float32 only")
+            rates = np.array([f.info.sample_rate for f in corpus.index.files] or [0], dtype=np.uint32)
+            _check(L.clx_batch_create_resampled_packed(self.ctx._h, corpus._h, rates.ctypes.data, len(corpus.index),
+                                                       self.max_excerpts, self.max_samples, self.sample_rate,
+                                                       C.byref(h)), self.ctx)
         self._batch = _Batch(self.ctx, h, keep=corpus)
         self.channels = corpus.channels
         self.stride = int(L.clx_batch_packed_stride(h))
@@ -1440,14 +1469,20 @@ class PackedBatch:
         if kind == 0:
             if not 0 <= fi < len(self.corpus.index):
                 raise ValueError(f"excerpt {b}: file index {fi} out of range")
-            N = self.corpus.index[fi].length
+            f = self.corpus.index[fi]
+            N, at = f.length, ""
+            if self.sample_rate is not None and f.info.sample_rate != self.sample_rate:
+                g = math.gcd(f.info.sample_rate, self.sample_rate)
+                N = -(-f.length * (self.sample_rate // g) // (f.info.sample_rate // g))
+                at = f" at {self.sample_rate} Hz"
             if not 0 <= o <= N:
-                raise ValueError(f"excerpt {b}: offset {o} outside file {fi} ({N} samples)")
+                raise ValueError(f"excerpt {b}: offset {o} outside file {fi} ({N} samples{at})")
             if ln == 0 or ln < -1:
                 raise ValueError(f"excerpt {b}: length {ln} (must be >= 1, or -1 for the rest of the file)")
             start = int(self._starts[b].item())
             n = N - o if ln == -1 else min(ln, N - o)
-            raise ValueError(f"excerpt {b}: needs columns [{start}, {start + n}), past max_samples {self.max_samples}")
+            raise ValueError(f"excerpt {b}: needs columns [{start}, {start + n}){at}, past max_samples "
+                             f"{self.max_samples}")
         raise Error(st, f"file {fi}, excerpt {b}")
 
     def kernel_ms(self) -> float:

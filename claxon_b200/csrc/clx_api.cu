@@ -236,7 +236,9 @@ struct clx_batch {
     clx::PackedBuffers packed{};
     // Resampled crop batches (clx_batch_create_resampled_crops): crop batches whose graph runs `inner`, a packed batch,
     // between the map and filter kernels.  crop.requests and crop.lengths are their own, crop.status and crop.error
-    // the inner batch's; buf.conv is the output; rs the rest.
+    // the inner batch's; buf.conv is the output; rs the rest.  Resampled packed batches
+    // (clx_batch_create_resampled_packed) are those with `packed` set too: packed holds their own requests, count and
+    // target column starts (its other buffers stay null), and crop.requests is null.
     clx_batch* inner = nullptr;
     clx::ResampleBuffers rs{};
 };
@@ -684,6 +686,13 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
 
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
     const clx::DecodeBuffers db = b->buf.view(b->n_frames, b->mode, b->stride);
+    if (b->inner && b->is_packed) {
+        const clx::CropCorpus cc = b->corpus->view(0);
+        cudaError_t e = clx::launch_resample_packed_map(cc, b->rs, b->packed, st, launches);
+        if (e == cudaSuccess) e = launch_batch(b->inner, st, launches);
+        if (e == cudaSuccess) e = clx::launch_resample_packed(b->rs, b->packed, st, launches);
+        return e;
+    }
     if (b->inner) {
         const clx::CropCorpus cc = b->corpus->view(0);
         cudaError_t e = clx::launch_resample_map(cc, b->rs, st, launches);
@@ -1349,6 +1358,73 @@ int clx_batch_create_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uin
         return cuda_fail(ctx, e, "clx_batch_create_resampled_crops");
     }
     rs.requests = cb.requests;
+    rs.lengths = cb.lengths;
+    rs.out = reinterpret_cast<float*>(b->buf.conv);
+    build_graph(ctx, b);
+    *out = b;
+    return CLX_OK;
+}
+
+int clx_batch_create_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                                      size_t max_excerpts, size_t max_samples, uint32_t target_rate, clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (!ctx || !corpus || !file_rates || n_files != corpus->n_files || max_excerpts == 0 || max_samples == 0 ||
+        max_excerpts >= (1u << 30) || max_samples > SIZE_MAX / 16)
+        return CLX_ERR_INVALID_ARGUMENT;
+    clx::ResampleTables t;
+    if (!clx::resample_tables(file_rates, n_files, target_rate, max_samples, &t)) return CLX_ERR_INVALID_ARGUMENT;
+    // The inner packed batch: the source spans of any excerpts that fit in T columns at R fit in its columns.
+    const size_t src_cols = clx::resample_packed_bound(t, max_excerpts, max_samples);
+    const size_t C = corpus->channels, stride = (max_samples + 3) & ~(size_t)3;
+    if (src_cols == SIZE_MAX || stride > (SIZE_MAX / 4 - 8) / C || (stride + t.tile - 1) / t.tile >= (1u << 31))
+        return CLX_ERR_INVALID_ARGUMENT;
+    clx_batch* inner = nullptr;
+    const int rc = clx_batch_create_packed(ctx, corpus, max_excerpts, src_cols, CLX_OUT_CHANNELS_F32, &inner);
+    if (rc != CLX_OK) return rc;
+    clx_batch* b = new clx_batch();
+    b->corpus = corpus;
+    corpus->live++;
+    b->inner = inner;
+    b->is_packed = true;
+    b->out_elems = C * stride;
+    b->mode = CLX_OUT_CHANNELS_F32;
+    b->stride = stride;
+    clx::CropBuffers& cb = b->crop;
+    cb.n_crops = (uint32_t)max_excerpts;
+    cb.C = (uint32_t)C;
+    cb.L = stride;
+    cb.status = inner->crop.status;
+    cb.error = inner->crop.error;
+    clx::PackedBuffers& pb = b->packed;
+    pb.T = max_samples;
+    clx::ResampleBuffers& rs = b->rs;
+    rs.n_crops = (uint32_t)max_excerpts;
+    rs.C = (uint32_t)C;
+    rs.L = stride;
+    rs.tile = t.tile;
+    rs.excerpts = const_cast<clx_packed_request*>(inner->packed.requests);
+    rs.count = const_cast<uint32_t*>(inner->packed.count);
+    rs.starts = inner->packed.starts;
+    rs.src = static_cast<const float*>((const void*)inner->buf.conv);
+    rs.src_stride = inner->stride;
+    cudaError_t e = cudaSetDevice(ctx->device);
+    if (e == cudaSuccess) e = device_zeros(pb.requests, max_excerpts);
+    if (e == cudaSuccess) e = device_zeros(pb.count, 1);
+    if (e == cudaSuccess) e = device_zeros(pb.starts, max_excerpts);
+    if (e == cudaSuccess) e = device_zeros(cb.lengths, max_excerpts);
+    if (e == cudaSuccess) e = device_zeros(b->buf.conv, (b->out_elems + 8) * sizeof(float));  // (the slack of fit())
+    if (e == cudaSuccess) e = cudaMalloc((void**)&rs.plan, max_excerpts * sizeof(clx::ResamplePlan));
+    if (e == cudaSuccess) e = upload(rs.file_rate, t.file_rate);
+    if (e == cudaSuccess) e = upload(rs.rates, t.rates);
+    if (e == cudaSuccess) e = upload(rs.coefs, t.coefs);
+    if (e == cudaSuccess) e = upload(rs.k0, t.k0);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
+    if (e != cudaSuccess) {
+        clx_batch_destroy(ctx, b);
+        return cuda_fail(ctx, e, "clx_batch_create_resampled_packed");
+    }
     rs.lengths = cb.lengths;
     rs.out = reinterpret_cast<float*>(b->buf.conv);
     build_graph(ctx, b);

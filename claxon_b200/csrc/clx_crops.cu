@@ -26,11 +26,11 @@
 
 #include "claxon_b200.h"
 #include "clx_internal.h"
+#include "clx_scan.cuh"
 
 namespace clx {
 
 constexpr uint32_t CROP_THREADS = 256;
-constexpr uint32_t SCAN_THREADS = 1024;
 
 // The frames of a file, [f0, f1), that overlap its samples [lo, hi), lo < hi <= its length: the first of them in
 // *first, their number returned (plan_range in claxon_b200/__init__.py does the same on the host).
@@ -351,50 +351,6 @@ packed_count_kernel(CropCorpus cc, CropBuffers cb, PackedBuffers pb) {
     cb.plan[b] = p;
     cb.lengths[b] = len;
     cb.status[b] = st;
-}
-
-// What packed_scan_kernel adds up: columns, slots, staging bytes and gather chunks.
-struct PackedSums {
-    uint64_t cols, bytes;
-    uint32_t slots, chunks;
-    __device__ PackedSums operator+(const PackedSums& o) const {
-        return {cols + o.cols, bytes + o.bytes, slots + o.slots, chunks + o.chunks};
-    }
-};
-
-__device__ __forceinline__ PackedSums shfl_up(const PackedSums& x, uint32_t o) {
-    return {__shfl_up_sync(0xffffffffu, x.cols, o), __shfl_up_sync(0xffffffffu, x.bytes, o),
-            __shfl_up_sync(0xffffffffu, x.slots, o), __shfl_up_sync(0xffffffffu, x.chunks, o)};
-}
-
-// Exclusive scan of v over the CTA (SCAN_THREADS threads, all of them call it), after *carry; *carry then includes the
-// whole CTA's sum.
-__device__ __forceinline__ PackedSums cta_scan(PackedSums v, PackedSums* s_warp, PackedSums* carry) {
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    PackedSums x = v;
-#pragma unroll
-    for (uint32_t o = 1; o < 32; o <<= 1) {
-        const PackedSums y = shfl_up(x, o);
-        if (lane >= o) x = x + y;
-    }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        PackedSums w = s_warp[lane];
-#pragma unroll
-        for (uint32_t o = 1; o < 32; o <<= 1) {
-            const PackedSums y = shfl_up(w, o);
-            if (lane >= o) w = w + y;
-        }
-        s_warp[lane] = w;
-    }
-    __syncthreads();
-    const PackedSums before = *carry + (warp ? s_warp[warp - 1] : PackedSums{}) + x;
-    const PackedSums excl{before.cols - v.cols, before.bytes - v.bytes, before.slots - v.slots, before.chunks - v.chunks};
-    __syncthreads();
-    if (threadIdx.x == SCAN_THREADS - 1) *carry = before;
-    __syncthreads();
-    return excl;
 }
 
 // One CTA, SCAN_THREADS excerpts at a time.  Columns first: start_b is the scan of round_up_4(n_b) over the valid

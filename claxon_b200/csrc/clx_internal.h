@@ -217,6 +217,15 @@ bool resample_tables(const uint32_t* file_rates, size_t n_files, uint32_t target
 // The two kernels around the packed batch's launch sequence.
 cudaError_t launch_resample_map(const CropCorpus& cc, const ResampleBuffers& rs, cudaStream_t stream, uint64_t* launches);
 cudaError_t launch_resample(const ResampleBuffers& rs, cudaStream_t stream, uint64_t* launches);
+// Resampled packed batches (clx_batch_create_resampled_packed) keep the same ResampleBuffers, with n_crops =
+// max_excerpts, L = the output's row stride and lengths at rate R, and their own PackedBuffers: the caller's requests
+// and count at rate R, the target column starts and T.  The inner packed batch has resample_packed_bound columns
+// (clx_resample_packed_source_bound over t's rates).
+size_t resample_packed_bound(const ResampleTables& t, size_t max_excerpts, size_t max_samples);
+cudaError_t launch_resample_packed_map(const CropCorpus& cc, const ResampleBuffers& rs, const PackedBuffers& pb,
+                                       cudaStream_t stream, uint64_t* launches);
+cudaError_t launch_resample_packed(const ResampleBuffers& rs, const PackedBuffers& pb, cudaStream_t stream,
+                                   uint64_t* launches);
 #ifdef CLX_EXPERIMENT
 extern int g_exp_which;  // measurement builds only: bit 0 = index pass, bit 1 = decode pass of LanePerFrame
 extern int g_exp_dyn_smem;

@@ -492,6 +492,36 @@ int clx_batch_create_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uin
  * target, else (floor((num_frames - 1) / n) + 2) * o + 2w.  SIZE_MAX if that overflows; 0 for a zero argument or a rate
  * above CLX_MAX_SAMPLE_RATE.  Host only. */
 size_t clx_resample_source_bound(uint32_t orig, uint32_t target, size_t num_frames);
+/* Resampled packed batches: packed batches of a corpus whose files may have different sample rates, every excerpt at one
+ * target rate R, with the filter of clx_batch_create_resampled_crops.  Everything counts samples at R: offsets, lengths,
+ * max_samples (T), the column starts and the returned lengths.  Excerpt b of request {file, 0, offset, length} is
+ * resample(x, r, R)[:, offset : offset + n_b], x the whole file, with n_b = min(length, N_t - offset) (N_t - offset for
+ * a length of -1); so the samples near an excerpt's edges are those of the resampled file.  The layout is
+ * clx_batch_create_packed's: start_0 = 0 and start_{b+1} = start_b + round_up_4(n_b) over the valid requests, those
+ * that do not fit included.  A request with file >= n_files, reserved != 0, offset < 0 or > N_t, or a length of 0 or
+ * below -1 is invalid; an excerpt with start_b + n_b > T does not fit; both get status CLX_ERR_INVALID_ARGUMENT, length
+ * 0, no columns and kind 0 in the error word.  offset == N_t is the valid empty excerpt.  A valid excerpt's status is
+ * that of its source span, as for resampled crops.  A file with r == R is copied, not filtered: over a corpus whose
+ * files are all at R, output, starts, lengths, status and error word are clx_batch_create_packed's (CLX_OUT_CHANNELS_F32)
+ * bit for bit.
+ * The output is [C, stride] float32 with stride = round_up_4(T); every element no excerpt covers reads 0 after every
+ * call (alignment gaps, rows a file does not have, the columns past the last excerpt and [T, stride)).  The packed
+ * accessors return the batch's own requests (clx_packed_request at rate R), count and target column starts, and the
+ * stride; clx_batch_crop_status / _error return the inner packed batch's, clx_batch_crop_lengths the lengths at R.
+ * Each call runs a kernel that lays the excerpts out at R and maps each one that fits to its source span, the launch
+ * sequence of an inner packed batch of clx_resample_packed_source_bound columns, and the filter kernel, which writes
+ * every element of the output.  CLX_ERR_INVALID_ARGUMENT for what clx_batch_create_resampled_crops refuses (its rates,
+ * its coefficient limit, sizes that overflow), for what clx_batch_create_packed refuses at the inner batch's size, and
+ * for max_excerpts 0 or 2^30 or more and max_samples 0. */
+int clx_batch_create_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                                      size_t max_excerpts, size_t max_samples, uint32_t target_rate, clx_batch** out);
+/* The inner packed batch's columns of a resampled packed batch: at least sum_b round_up_4(span_b) over any excerpts
+ * that fit in max_samples (T) columns at target_rate, span_b an excerpt's source span.  An excerpt of m >= 1 outputs has
+ * round_up_4(span) <= (r / R) m + c_r, c_r = 2o + 2w + 3 for r != R and 3 for r == R, and at most k = min(max_excerpts,
+ * T) excerpts have outputs, m's adding up to T at most: ceil(T * max r / R) + k * max c_r, rounded up to 4.  SIZE_MAX if
+ * that overflows; 0 for a zero argument, a rate above CLX_MAX_SAMPLE_RATE or no file_rates for n_files > 0.  Host only. */
+size_t clx_resample_packed_source_bound(const uint32_t* file_rates, size_t n_files, uint32_t target_rate,
+                                        size_t max_excerpts, size_t max_samples);
 int clx_batch_decode(clx_ctx* ctx, clx_batch* b, uint32_t stream_index); /* async on an internal stream */
 int clx_batch_sync(clx_ctx* ctx, clx_batch* b);
 /* Planar batches only (CLX_ERR_INVALID_ARGUMENT for any other mode). */

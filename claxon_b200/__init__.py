@@ -24,12 +24,12 @@ from ._lib import (OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT)
 from ._lib import (FrameDesc, FrameResult, FrameWindow, OPT_NO_VERIFY_CRC, OPT_GENERIC_KERNEL_ONLY, OPT_WARP_PER_FRAME, OPT_LANE_PER_FRAME,
                    OPT_NO_GENERIC, OPT_NO_WIDE, FRAME_VARIABLE_BLOCKING, FRAME_CRC16_VERIFIED,
                    OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24,
-                   OUT_CHANNELS_I32, OUT_CHANNELS_F32)
+                   OUT_CHANNELS_I32, OUT_CHANNELS_F32, MEL_CENTER, MEL_LOG)
 
 __all__ = ["Error", "Block", "FrameReader", "FlacReader", "FlacReaderOptions", "StreamInfo", "Context", "DeviceBatch",
            "parse_frame_header", "demux_frames", "open_stream", "ogg_frames", "mp4_frames", "status_str", "DESC_DTYPE", "RESULT_DTYPE", "load", "plan_columns",
            "WINDOW_DTYPE", "index", "FlacIndex", "IndexedFile", "load_crops", "plan_range", "frame_starts", "Corpus",
-           "CropBatch", "PackedBatch"]
+           "CropBatch", "PackedBatch", "MelCropBatch", "melscale_fbanks"]
 
 # numpy views of the C structs (same layout; asserted below)
 DESC_DTYPE = np.dtype([
@@ -1030,6 +1030,19 @@ class Corpus:
         R, every crop is at rate R whatever its file's rate: offsets and num_frames count samples at R (see CropBatch)."""
         return CropBatch(self, batch, num_frames, dtype, sample_rate)
 
+    def mel_crops(self, batch: int, num_frames: int, sample_rate: int | None = None, *, n_fft: int = 400,
+                  win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
+                  f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
+                  center: bool = True, norm: str | None = None, mel_scale: str = "htk",
+                  log_floor: float | None = None) -> "MelCropBatch":
+        """A MelCropBatch: the mel spectrogram of each crop of a crop batch of `batch` crops of `num_frames` samples
+        (resampled to `sample_rate` when given), computed on the device.  The keywords are those of
+        torchaudio.transforms.MelSpectrogram (window_fn None is torch.hann_window); log_floor None gives the power,
+        a float ln(max(mel, log_floor))."""
+        return MelCropBatch(self, batch, num_frames, sample_rate, n_fft=n_fft, win_length=win_length,
+                            hop_length=hop_length, f_min=f_min, f_max=f_max, n_mels=n_mels, window_fn=window_fn,
+                            wkwargs=wkwargs, center=center, norm=norm, mel_scale=mel_scale, log_floor=log_floor)
+
     def resample_source_bound(self, num_frames: int, sample_rate: int) -> int:
         """The most source samples a crop of num_frames samples at `sample_rate` reads from one file of the corpus
         (clx_resample_source_bound, the largest over the files' rates)."""
@@ -1273,11 +1286,16 @@ class CropBatch:
             _check(L.clx_batch_create_resampled_crops(self.ctx._h, corpus._h, rates.ctypes.data, len(corpus.index),
                                                       self.batch, self.num_frames, self.sample_rate, C.byref(h)),
                    self.ctx)
-        self._batch = _Batch(self.ctx, h, keep=corpus)
         self.channels = corpus.channels
+        self._attach(h, (self.batch, self.channels, self.num_frames), "<f4" if mode == OUT_CHANNELS_F32 else "<i4")
+
+    def _attach(self, h, out_shape: tuple, typestr: str):
+        """Takes ownership of the created batch `h` and views its buffers: out, lengths, status, requests, error."""
+        import torch
+        L = self.ctx._L
+        self._batch = _Batch(self.ctx, h, keep=self.corpus)
         B, view = self.batch, self._batch.tensor
-        self.out = view(L.clx_batch_device_out(h), (B, self.channels, self.num_frames),
-                        "<f4" if mode == OUT_CHANNELS_F32 else "<i4")
+        self.out = view(L.clx_batch_device_out(h), out_shape, typestr)
         self.lengths = view(L.clx_batch_crop_lengths(h), (B,), "<i8")
         self.status = view(L.clx_batch_crop_status(h), (B,), "<i4")
         self._requests = view(L.clx_batch_crop_requests(h), (B, 2), "<i8")  # {u32 file, u32 reserved} as one i64, offset
@@ -1339,6 +1357,122 @@ class CropBatch:
     def kernel_ms(self) -> float:
         """Device time of the last call's graph (CUDA events), planner and status pass included."""
         return self._batch.kernel_ms()
+
+
+def _hz_to_mel(f, mel_scale: str):
+    f = np.asarray(f, dtype=np.float64)
+    if mel_scale == "htk":
+        return 2595.0 * np.log10(1.0 + f / 700.0)
+    f_sp, min_log_hz, logstep = 200.0 / 3, 1000.0, math.log(6.4) / 27.0
+    with np.errstate(divide="ignore"):
+        return np.where(f >= min_log_hz, min_log_hz / f_sp + np.log(f / min_log_hz) / logstep, f / f_sp)
+
+
+def _mel_to_hz(m, mel_scale: str):
+    m = np.asarray(m, dtype=np.float64)
+    if mel_scale == "htk":
+        return 700.0 * (10.0 ** (m / 2595.0) - 1.0)
+    f_sp, min_log_hz, logstep = 200.0 / 3, 1000.0, math.log(6.4) / 27.0
+    min_log_mel = min_log_hz / f_sp
+    return np.where(m >= min_log_mel, min_log_hz * np.exp(logstep * (m - min_log_mel)), f_sp * m)
+
+
+def melscale_fbanks(n_freqs: int, f_min: float, f_max: float, n_mels: int, sample_rate: int, norm: str | None = None,
+                    mel_scale: str = "htk") -> np.ndarray:
+    """torchaudio.functional.melscale_fbanks in float64 numpy: the [n_freqs, n_mels] triangular filterbank over the
+    bins linspace(0, sample_rate // 2, n_freqs), its corners equally spaced on the HTK or Slaney mel scale from f_min to
+    f_max; norm "slaney" divides each triangle by half its width in Hz."""
+    if norm not in (None, "slaney"):
+        raise ValueError('norm must be None or "slaney"')
+    if mel_scale not in ("htk", "slaney"):
+        raise ValueError('mel_scale must be "htk" or "slaney"')
+    all_freqs = np.linspace(0.0, float(int(sample_rate) // 2), int(n_freqs))
+    m_pts = np.linspace(float(_hz_to_mel(f_min, mel_scale)), float(_hz_to_mel(f_max, mel_scale)), int(n_mels) + 2)
+    f_pts = _mel_to_hz(m_pts, mel_scale)
+    f_diff = f_pts[1:] - f_pts[:-1]
+    slopes = f_pts[None, :] - all_freqs[:, None]
+    fb = np.maximum(0.0, np.minimum(-slopes[:, :-2] / f_diff[:-1], slopes[:, 2:] / f_diff[1:]))
+    if norm == "slaney":
+        fb *= (2.0 / (f_pts[2:n_mels + 2] - f_pts[:n_mels]))[None, :]
+    return fb
+
+
+def _mel_rate(index: FlacIndex, sample_rate: int | None) -> int:
+    """The filterbank's rate: `sample_rate` when given, else the corpus's one STREAMINFO rate."""
+    if sample_rate is not None:
+        return int(sample_rate)
+    rates = {f.info.sample_rate for f in index.files}
+    if len(rates) != 1:
+        raise ValueError(f"a corpus of {len(rates)} sample rates needs sample_rate= for its mel spectrogram")
+    return rates.pop()
+
+
+def _mel_tables(sample_rate: int, n_fft: int, win_length, hop_length, f_min: float, f_max, n_mels: int, window_fn,
+                wkwargs, center: bool, norm, mel_scale: str, log_floor):
+    """MelSpectrogram's arguments as (clx_mel_params, window [win_length] float32, fbank [n_fft // 2 + 1, n_mels]
+    float32); the C ABI checks the ranges."""
+    import torch
+    n_fft, n_mels = int(n_fft), int(n_mels)
+    win_length = n_fft if win_length is None else int(win_length)
+    hop_length = win_length // 2 if hop_length is None else int(hop_length)
+    f_max = float(sample_rate // 2) if f_max is None else float(f_max)
+    flags = MEL_CENTER if center else 0
+    if log_floor is not None:
+        log_floor = float(log_floor)
+        if not (math.isfinite(log_floor) and log_floor > 0):
+            raise ValueError("log_floor must be finite and > 0")
+        flags |= MEL_LOG
+    if min(n_fft, win_length, hop_length, n_mels) < 1:
+        raise ValueError("n_fft, win_length, hop_length and n_mels must be >= 1")
+    window = (torch.hann_window if window_fn is None else window_fn)(win_length, **(wkwargs or {}))
+    window = np.ascontiguousarray(torch.as_tensor(window).detach().cpu().numpy(), dtype=np.float32).reshape(-1)
+    if window.size != win_length:
+        raise ValueError(f"window_fn gave {window.size} values for win_length {win_length}")
+    fbank = np.ascontiguousarray(melscale_fbanks(n_fft // 2 + 1, f_min, f_max, n_mels, sample_rate, norm, mel_scale),
+                                 dtype=np.float32)
+    params = _lib.MelParams(n_fft, win_length, hop_length, n_mels, flags, 0.0 if log_floor is None else log_floor)
+    return params, window, fbank
+
+
+class MelCropBatch(CropBatch):
+    """The mel spectrogram of every crop of a crop batch, computed on the device inside the batch's CUDA graph
+    (clx_batch_create_mel_crops): a call returns (features [B, C, n_mels, F] float32, lengths [B] int64), with the
+    requests, `status`, check, stream and sync rules of CropBatch.
+
+    features = MelSpectrogram(x), x the [B, C, L] float32 output of the equivalent CropBatch (the resampled one with
+    `sample_rate`) for the same requests, MelSpectrogram being torchaudio.transforms.MelSpectrogram(rate, n_fft=...,
+    ...) with power 2, pad_mode "reflect", applied to x as a tensor: each crop is reflect-padded with its own samples,
+    and its zero columns and rows are transformed like any others.  F = 1 + L // hop_length with center, else 1 + (L -
+    n_fft) // hop_length.  With log_floor, features = ln(max(mel, log_floor)).  An invalid request's features are 0
+    (ln(log_floor) with the log); a failed crop's are unspecified.  lengths and status are the crop batch's, lengths in
+    samples at the crop's rate.  The filterbank's rate is `sample_rate`, else the corpus's single rate (ValueError for
+    a corpus of mixed rates).  n_fft must be even, 8 to 4096, with n_fft / 2 a product of 2, 3 and 5; n_mels at most
+    512; L above n_fft / 2 with center, at least n_fft without (Error 90 otherwise)."""
+
+    def __init__(self, corpus: Corpus, batch: int, num_frames: int, sample_rate: int | None = None, *,
+                 n_fft: int = 400, win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
+                 f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
+                 center: bool = True, norm: str | None = None, mel_scale: str = "htk", log_floor: float | None = None):
+        import torch
+        self.corpus, self.ctx = corpus, corpus.ctx
+        self.batch, self.num_frames, self.dtype = int(batch), int(num_frames), torch.float32
+        self.sample_rate = None if sample_rate is None else int(sample_rate)
+        if self.batch < 1 or self.num_frames < 1:
+            raise ValueError("batch and num_frames must be >= 1")
+        params, window, fbank = _mel_tables(_mel_rate(corpus.index, self.sample_rate), n_fft, win_length, hop_length,
+                                            f_min, f_max, n_mels, window_fn, wkwargs, center, norm, mel_scale,
+                                            log_floor)
+        self.params, self.fbank, self.window = params, fbank, window
+        L = self.ctx._L
+        rates = np.array([f.info.sample_rate for f in corpus.index.files] or [0], dtype=np.uint32)
+        h = C.c_void_p()
+        _check(L.clx_batch_create_mel_crops(self.ctx._h, corpus._h, rates.ctypes.data, len(corpus.index), self.batch,
+                                            self.num_frames, self.sample_rate or 0, C.byref(params),
+                                            window.ctypes.data, fbank.ctypes.data, C.byref(h)), self.ctx)
+        self.channels, self.n_mels = corpus.channels, params.n_mels
+        self.n_frames = (1 + self.num_frames // params.hop_length if center else
+                         1 + (self.num_frames - params.n_fft) // params.hop_length)
+        self._attach(h, (self.batch, self.channels, self.n_mels, self.n_frames), "<f4")
 
 
 def _request_column(x, n: int | None, what: str):

@@ -55,8 +55,14 @@ class ImageFile(C.Structure):  # clx_image_file: one file's record in a corpus i
                 ("first_frame", C.c_uint32), ("n_frames", C.c_uint32), ("flags", C.c_uint32), ("tail", C.c_int32)]
 
 
+class MelParams(C.Structure):  # clx_mel_params
+    _fields_ = [("n_fft", C.c_uint32), ("win_length", C.c_uint32), ("hop_length", C.c_uint32), ("n_mels", C.c_uint32),
+                ("flags", C.c_uint32), ("log_floor", C.c_float)]
+
+
 assert C.sizeof(FrameDesc) == 40 and C.sizeof(FrameResult) == 8 and C.sizeof(FrameWindow) == 16
 assert C.sizeof(StreamInfoC) == 56 and C.sizeof(ImageHeader) == 96 and C.sizeof(ImageFile) == 88
+assert C.sizeof(MelParams) == 24
 
 OPT_NO_VERIFY_CRC = 1
 OPT_GENERIC_KERNEL_ONLY = 2
@@ -67,6 +73,7 @@ OPT_NO_WIDE = 32
 OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT = 1, 2
 BATCH_BYTES_ON_DEVICE = 1
 CORPUS_HOST = 1
+MEL_CENTER, MEL_LOG = 1, 2
 IMAGE_MAGIC, IMAGE_VERSION, IMAGE_ALIGN, IMAGE_END_CONFIRMED = 0x3150524F43584C43, 1, 4096, 1
 OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24 = 0, 1, 2, 3
 OUT_CHANNELS_I32, OUT_CHANNELS_F32 = 4, 5
@@ -131,6 +138,7 @@ SYMBOLS = {
     "clx_resample_source_bound": (_sz, [C.c_uint32, C.c_uint32, _sz]),
     "clx_batch_create_resampled_packed": (C.c_int, [_vp, _vp, _vp, _sz, _sz, _sz, C.c_uint32, C.POINTER(_vp)]),
     "clx_resample_packed_source_bound": (_sz, [_vp, _sz, C.c_uint32, _sz, _sz]),
+    "clx_batch_create_mel_crops": (C.c_int, [_vp, _vp, _vp, _sz, _sz, _sz, C.c_uint32, _vp, _vp, _vp, C.POINTER(_vp)]),
     "clx_batch_decode": (C.c_int, [_vp, _vp, C.c_uint32]),
     "clx_batch_sync": (C.c_int, [_vp, _vp]),
     "clx_batch_read": (C.c_int, [_vp, _vp, _vp, _sz, _vp]),

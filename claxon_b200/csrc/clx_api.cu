@@ -10,6 +10,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cmath>
 #include <condition_variable>
 #include <functional>
 #include <map>
@@ -241,6 +242,11 @@ struct clx_batch {
     // target column starts (its other buffers stay null), and crop.requests is null.
     clx_batch* inner = nullptr;
     clx::ResampleBuffers rs{};
+    // Mel crop batches (clx_batch_create_mel_crops): `inner` is a crop or resampled crop batch, run before mel_kernel.
+    // crop.requests, status, lengths and error are the inner batch's; buf.conv is the features; mel the rest.
+    bool is_mel = false;
+    clx::MelBuffers mel{};
+    size_t mel_smem = 0;
 };
 
 struct clx_corpus {
@@ -686,6 +692,11 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
 
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
     const clx::DecodeBuffers db = b->buf.view(b->n_frames, b->mode, b->stride);
+    if (b->is_mel) {
+        cudaError_t e = launch_batch(b->inner, st, launches);
+        if (e == cudaSuccess) e = clx::launch_mel(b->mel, b->mel_smem, st, launches);
+        return e;
+    }
     if (b->inner && b->is_packed) {
         const clx::CropCorpus cc = b->corpus->view(0);
         cudaError_t e = clx::launch_resample_packed_map(cc, b->rs, b->packed, st, launches);
@@ -828,6 +839,12 @@ void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
     (void)ctx;
     if (!b) return;
     b->buf.release();
+    if (b->is_mel) {
+        b->crop.requests = nullptr;  // the inner batch's, as status and error below
+        b->crop.lengths = nullptr;
+        cudaFree((void*)b->mel.tw); cudaFree((void*)b->mel.window); cudaFree((void*)b->mel.bands);
+        cudaFree((void*)b->mel.weights);
+    }
     if (b->inner) {
         b->crop.status = nullptr;  // the inner batch's
         b->crop.error = nullptr;
@@ -1427,6 +1444,70 @@ int clx_batch_create_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const ui
     }
     rs.lengths = cb.lengths;
     rs.out = reinterpret_cast<float*>(b->buf.conv);
+    build_graph(ctx, b);
+    *out = b;
+    return CLX_OK;
+}
+
+int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                               size_t n_crops, size_t num_frames, uint32_t target_rate, const clx_mel_params* params,
+                               const float* window, const float* fbank, clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (!ctx || !corpus || n_crops == 0 || n_crops >= (1u << 30)) return CLX_ERR_INVALID_ARGUMENT;
+    clx::MelTables t;
+    if (!clx::mel_tables(params, window, fbank, num_frames, &t)) return CLX_ERR_INVALID_ARGUMENT;
+    const size_t C = corpus->channels, rows = n_crops * C;  // (< 2^33: no overflow)
+    const uint64_t tiles = (t.F + t.tile - 1) / t.tile;
+    if (t.F > (SIZE_MAX / 4 - 8) / (rows * params->n_mels) || tiles >= (1u << 31) / rows) return CLX_ERR_INVALID_ARGUMENT;
+    clx_batch* inner = nullptr;
+    const int rc = target_rate ? clx_batch_create_resampled_crops(ctx, corpus, file_rates, n_files, n_crops, num_frames,
+                                                                  target_rate, &inner)
+                               : clx_batch_create_crops(ctx, corpus, n_crops, num_frames, CLX_OUT_CHANNELS_F32, &inner);
+    if (rc != CLX_OK) return rc;
+    clx_batch* b = new clx_batch();
+    b->corpus = corpus;
+    corpus->live++;
+    b->inner = inner;
+    b->is_mel = true;
+    b->out_elems = rows * params->n_mels * t.F;
+    b->mode = CLX_OUT_CHANNELS_F32;
+    b->stride = t.F;
+    b->crop.requests = inner->crop.requests;
+    b->crop.status = inner->crop.status;
+    b->crop.lengths = inner->crop.lengths;
+    b->crop.error = inner->crop.error;
+    b->crop.n_crops = (uint32_t)n_crops;
+    b->crop.C = (uint32_t)C;
+    b->crop.L = num_frames;
+    clx::MelBuffers& mb = b->mel;
+    mb.src = reinterpret_cast<const float*>(inner->buf.conv);
+    mb.L = num_frames;
+    mb.F = t.F;
+    mb.rows = (uint32_t)rows;
+    mb.tiles = (uint32_t)tiles;
+    mb.n_fft = params->n_fft;
+    mb.hop = params->hop_length;
+    mb.n_mels = params->n_mels;
+    mb.tile = t.tile;
+    mb.flags = params->flags;
+    mb.log_floor = params->log_floor;
+    mb.log_of_floor = (params->flags & CLX_MEL_LOG) ? (float)std::log((double)params->log_floor) : 0.f;
+    b->mel_smem = t.smem;
+    cudaError_t e = cudaSetDevice(ctx->device);
+    if (e == cudaSuccess) e = clx::mel_init();
+    if (e == cudaSuccess) e = device_zeros(b->buf.conv, (b->out_elems + 8) * sizeof(float));  // (the slack of fit())
+    if (e == cudaSuccess) e = upload(mb.tw, t.tw);
+    if (e == cudaSuccess) e = upload(mb.window, t.window);
+    if (e == cudaSuccess) e = upload(mb.bands, t.bands);
+    if (e == cudaSuccess) e = upload(mb.weights, t.weights);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
+    if (e != cudaSuccess) {
+        clx_batch_destroy(ctx, b);
+        return cuda_fail(ctx, e, "clx_batch_create_mel_crops");
+    }
+    mb.out = reinterpret_cast<float*>(b->buf.conv);
     build_graph(ctx, b);
     *out = b;
     return CLX_OK;

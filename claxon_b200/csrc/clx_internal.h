@@ -226,6 +226,37 @@ cudaError_t launch_resample_packed_map(const CropCorpus& cc, const ResampleBuffe
                                        cudaStream_t stream, uint64_t* launches);
 cudaError_t launch_resample_packed(const ResampleBuffers& rs, const PackedBuffers& pb, cudaStream_t stream,
                                    uint64_t* launches);
+
+// clx_mel.cu: mel crop batches (clx_batch_create_mel_crops), one kernel after an inner crop or resampled crop batch.
+// Mel m sums weights[w + i] * |X[lo + i]|^2 for i < n: the non-zero span of its filterbank column.
+struct MelBand {
+    uint32_t lo, n, w;
+};
+struct MelBuffers {
+    const float* src;       // the inner batch's [rows, L] output
+    float* out;             // [rows, n_mels, F]
+    const float* tw;        // n_fft complex: exp(-2 pi i k / n_fft)
+    const float* window;    // n_fft: the window at (n_fft - win_length) / 2, zeros around it
+    const MelBand* bands;   // n_mels
+    const float* weights;
+    uint64_t L, F;
+    uint32_t rows, tiles;   // CTAs: rows * tiles
+    uint32_t n_fft, hop, n_mels, tile;  // tile: frames per CTA
+    uint32_t flags;         // CLX_MEL_*
+    float log_floor, log_of_floor;  // ln(log_floor), taken in float64
+};
+// The host side of clx_batch_create_mel_crops: the checks of the header's refusals that do not depend on the inner
+// batch, the frame count F and the tables.  false for a refusal.
+struct MelTables {
+    std::vector<float> tw, window, weights;
+    std::vector<MelBand> bands;
+    uint64_t F = 0;
+    uint32_t tile = 0;
+    size_t smem = 0;
+};
+bool mel_tables(const clx_mel_params* p, const float* window, const float* fbank, size_t num_frames, MelTables* t);
+cudaError_t mel_init();  // mel_kernel's shared memory limit, on the current device, before a graph captures it
+cudaError_t launch_mel(const MelBuffers& mb, size_t smem, cudaStream_t stream, uint64_t* launches);
 #ifdef CLX_EXPERIMENT
 extern int g_exp_which;  // measurement builds only: bit 0 = index pass, bit 1 = decode pass of LanePerFrame
 extern int g_exp_dyn_smem;

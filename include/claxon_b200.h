@@ -522,6 +522,42 @@ int clx_batch_create_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const ui
  * that overflows; 0 for a zero argument, a rate above CLX_MAX_SAMPLE_RATE or no file_rates for n_files > 0.  Host only. */
 size_t clx_resample_packed_source_bound(const uint32_t* file_rates, size_t n_files, uint32_t target_rate,
                                         size_t max_excerpts, size_t max_samples);
+/* Mel crop batches: the mel spectrogram of every row of a crop batch, torchaudio.transforms.MelSpectrogram with power
+ * 2, normalized False, pad 0, onesided and pad_mode "reflect", optionally followed by a natural log.  The inner batch is
+ * clx_batch_create_crops(ctx, corpus, n_crops, num_frames, CLX_OUT_CHANNELS_F32) when target_rate is 0 (file_rates may
+ * then be NULL), else clx_batch_create_resampled_crops(ctx, corpus, file_rates, n_files, n_crops, num_frames,
+ * target_rate); x is its [n_crops * C, L] output (L = num_frames), zero columns and rows included.  For each row: with
+ * CLX_MEL_CENTER it is reflect-padded by n_fft / 2 on each side with its own samples, and F = 1 + L / hop_length; else
+ * F = 1 + (L - n_fft) / hop_length.  Frame t is samples [t * hop, t * hop + n_fft) of the (padded) row times the
+ * window's win_length values at offset (n_fft - win_length) / 2, zeros around them; mel[m, t] = sum_k fbank[k * n_mels
+ * + m] |X_t[k]|^2 over k <= n_fft / 2, X_t the DFT of the frame (fbank: torchaudio's melscale_fbanks layout, [n_fft / 2
+ * + 1][n_mels]); with CLX_MEL_LOG the output is ln(max(mel, log_floor)), ln(log_floor) taken in float64.  The output is
+ * [n_crops * C, n_mels, F] float32, element (r, m, t) at (r * n_mels + m) * F + t, written whole by each call: an
+ * invalid request's features are 0 (ln(log_floor) with the log), a failed crop's are unspecified.  The crop accessors
+ * (requests, status, lengths in samples at the crop's rate, error) return the inner batch's buffers;
+ * clx_batch_device_out, decode, sync, last_kernel_ms, read_to and clx_ctx_run_steps work on the mel batch.  Each call is
+ * the inner batch's launch sequence and one more kernel, which reads the inner output once per frame overlap and keeps
+ * the FFTs in shared memory: the batch holds the inner batch, the output and tables of a few times n_fft floats.  The
+ * power is computed in f32 from float64 tables, each mel summing only its bins of non-zero weight.
+ * CLX_ERR_INVALID_ARGUMENT for what the inner create refuses; NULL params, window or fbank; n_fft odd, below 8, above
+ * 4096 or with n_fft / 2 having a prime factor above 5; win_length 0 or above n_fft; hop_length 0; n_mels 0 or above
+ * 512; other flags; with CLX_MEL_LOG a log_floor that is not finite and > 0, without it one that is not 0; a window or
+ * fbank value that is not finite; num_frames <= n_fft / 2 with CLX_MEL_CENTER (torch.stft refuses that reflect pad),
+ * num_frames < n_fft without; sizes that overflow. */
+#define CLX_MEL_CENTER 1u  /* reflect-pad n_fft / 2 samples on each side (torch.stft center=True, pad_mode "reflect") */
+#define CLX_MEL_LOG 2u     /* store ln(max(mel, log_floor)) */
+typedef struct clx_mel_params {
+    uint32_t n_fft;       /* even, 8 .. 4096, n_fft / 2 with no prime factor above 5 (400, 512, 320, 480, 1024, 2048 ...) */
+    uint32_t win_length;  /* 1 .. n_fft */
+    uint32_t hop_length;  /* >= 1 */
+    uint32_t n_mels;      /* 1 .. 512 */
+    uint32_t flags;       /* CLX_MEL_* */
+    float log_floor;      /* > 0 and finite with CLX_MEL_LOG, else 0 */
+} clx_mel_params;
+int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                               size_t n_crops, size_t num_frames, uint32_t target_rate, const clx_mel_params* params,
+                               const float* window /* win_length */, const float* fbank /* [n_fft / 2 + 1][n_mels] */,
+                               clx_batch** out);
 int clx_batch_decode(clx_ctx* ctx, clx_batch* b, uint32_t stream_index); /* async on an internal stream */
 int clx_batch_sync(clx_ctx* ctx, clx_batch* b);
 /* Planar batches only (CLX_ERR_INVALID_ARGUMENT for any other mode). */

@@ -29,7 +29,7 @@ from ._lib import (FrameDesc, FrameResult, FrameWindow, OPT_NO_VERIFY_CRC, OPT_G
 __all__ = ["Error", "Block", "FrameReader", "FlacReader", "FlacReaderOptions", "StreamInfo", "Context", "DeviceBatch",
            "parse_frame_header", "demux_frames", "open_stream", "ogg_frames", "mp4_frames", "status_str", "DESC_DTYPE", "RESULT_DTYPE", "load", "plan_columns",
            "WINDOW_DTYPE", "index", "FlacIndex", "IndexedFile", "load_crops", "plan_range", "frame_starts", "Corpus",
-           "CropBatch", "PackedBatch", "MelCropBatch", "melscale_fbanks"]
+           "CropBatch", "PackedBatch", "MelCropBatch", "MelPackedBatch", "melscale_fbanks"]
 
 # numpy views of the C structs (same layout; asserted below)
 DESC_DTYPE = np.dtype([
@@ -1066,6 +1066,28 @@ class Corpus:
         max_samples and the starts count samples at R (see PackedBatch)."""
         return PackedBatch(self, max_excerpts, max_samples, dtype, sample_rate)
 
+    def mel_packed(self, max_excerpts: int, max_samples: int, sample_rate: int | None = None, *, n_fft: int = 400,
+                   win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
+                   f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
+                   center: bool = True, norm: str | None = None, mel_scale: str = "htk",
+                   log_floor: float | None = None) -> "MelPackedBatch":
+        """A MelPackedBatch: the mel spectrogram of each excerpt of a packed batch of up to `max_excerpts` excerpts
+        along `max_samples` columns (resampled to `sample_rate` when given), packed along frames, computed on the
+        device.  The keywords are mel_crops()'s."""
+        return MelPackedBatch(self, max_excerpts, max_samples, sample_rate, n_fft=n_fft, win_length=win_length,
+                              hop_length=hop_length, f_min=f_min, f_max=f_max, n_mels=n_mels, window_fn=window_fn,
+                              wkwargs=wkwargs, center=center, norm=norm, mel_scale=mel_scale, log_floor=log_floor)
+
+    def mel_packed_frames_bound(self, max_excerpts: int, max_samples: int, *, n_fft: int = 400,
+                                win_length: int | None = None, hop_length: int | None = None,
+                                center: bool = True) -> int:
+        """clx_mel_packed_frames_bound: the frame columns T_f of a MelPackedBatch with these parameters, which hold
+        the frames of any excerpts that fit in max_samples columns (about max_samples / hop_length + 4 per excerpt)."""
+        win_length = int(n_fft) if win_length is None else int(win_length)
+        hop_length = win_length // 2 if hop_length is None else int(hop_length)
+        params = _lib.MelParams(int(n_fft), win_length, hop_length, 1, MEL_CENTER if center else 0, 0.0)
+        return int(self.ctx._L.clx_mel_packed_frames_bound(C.byref(params), int(max_excerpts), int(max_samples)))
+
     def resample_packed_source_bound(self, max_excerpts: int, max_samples: int, sample_rate: int) -> int:
         """clx_resample_packed_source_bound: the columns of the packed batch that decodes the source spans of a
         resampled PackedBatch (about max_samples x r / R for the corpus's highest rate r)."""
@@ -1613,12 +1635,85 @@ class PackedBatch:
                 raise ValueError(f"excerpt {b}: offset {o} outside file {fi} ({N} samples{at})")
             if ln == 0 or ln < -1:
                 raise ValueError(f"excerpt {b}: length {ln} (must be >= 1, or -1 for the rest of the file)")
-            start = int(self._starts[b].item())
+            start = self._sample_start(b)
             n = N - o if ln == -1 else min(ln, N - o)
             raise ValueError(f"excerpt {b}: needs columns [{start}, {start + n}){at}, past max_samples "
                              f"{self.max_samples}")
         raise Error(st, f"file {fi}, excerpt {b}")
 
+    def _sample_start(self, b: int) -> int:
+        """Excerpt b's first column (one sync)."""
+        return int(self._starts[b].item())
+
     def kernel_ms(self) -> float:
         """Device time of the last call's graph (CUDA events), planner and status pass included."""
         return self._batch.kernel_ms()
+
+
+class MelPackedBatch(PackedBatch):
+    """The mel spectrogram of every excerpt of a packed batch, packed along frames and computed on the device inside
+    the batch's CUDA graph (clx_batch_create_mel_packed): a call returns (features [C, n_mels, T_f] float32, starts [n]
+    int64, frames [n] int64, lengths [n] int64), all views of the batch's own buffers, with the requests, `status`,
+    check, stream and sync rules of PackedBatch, and its raises (offsets, lengths and columns in samples at the
+    batch's rate).  The parameters are MelCropBatch's.
+
+    Take x [C, T], s_b and n_b the output, sample starts and lengths of the equivalent float32 PackedBatch (the
+    resampled one with `sample_rate`) for the same requests.  Excerpt b's F_b frames are MelSpectrogram(x[:, s_b : s_b +
+    n_b]), as MelCropBatch computes it: each excerpt is reflect-padded with its own samples at its own two edges, as
+    torchaudio does on what load(file, frame_offset=o, num_frames=n) returns, and rows its file does not have are zeros
+    transformed like any others (exactly 0, or ln(log_floor)).  F_b = 1 + n_b // hop_length with center when n_b >
+    n_fft / 2, 1 + (n_b - n_fft) // hop_length without when n_b >= n_fft, else 0: invalid, non-fitting, empty and too
+    short excerpts have no frames (a too short one keeps status 0 and its length in samples).  Excerpt b's frames are
+    columns [starts[b], starts[b] + frames[b]) of every (row, mel), starts[0] = 0 and starts[b + 1] = starts[b] +
+    round_up_4(frames[b]); every other element of the features reads exactly 0 after every call, with or without the
+    log.  T_f = Corpus.mel_packed_frames_bound(max_excerpts, max_samples, ...) holds the frames of any excerpts that fit
+    in max_samples columns, so only the packed batch's fit rule applies.  Calls are bit-identical.  Memory: the packed
+    batch and C x n_mels x T_f float32."""
+
+    def __init__(self, corpus: Corpus, max_excerpts: int, max_samples: int, sample_rate: int | None = None, *,
+                 n_fft: int = 400, win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
+                 f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
+                 center: bool = True, norm: str | None = None, mel_scale: str = "htk", log_floor: float | None = None):
+        import torch
+        self.corpus, self.ctx = corpus, corpus.ctx
+        self.max_excerpts, self.max_samples, self.dtype = int(max_excerpts), int(max_samples), torch.float32
+        self.sample_rate = None if sample_rate is None else int(sample_rate)
+        if self.max_excerpts < 1 or self.max_samples < 1:
+            raise ValueError("max_excerpts and max_samples must be >= 1")
+        params, window, fbank = _mel_tables(_mel_rate(corpus.index, self.sample_rate), n_fft, win_length, hop_length,
+                                            f_min, f_max, n_mels, window_fn, wkwargs, center, norm, mel_scale,
+                                            log_floor)
+        self.params, self.fbank, self.window = params, fbank, window
+        L = self.ctx._L
+        rates = np.array([f.info.sample_rate for f in corpus.index.files] or [0], dtype=np.uint32)
+        h = C.c_void_p()
+        _check(L.clx_batch_create_mel_packed(self.ctx._h, corpus._h, rates.ctypes.data, len(corpus.index),
+                                             self.max_excerpts, self.max_samples, self.sample_rate or 0,
+                                             C.byref(params), window.ctypes.data, fbank.ctypes.data, C.byref(h)),
+               self.ctx)
+        self._batch = _Batch(self.ctx, h, keep=corpus)
+        self.channels, self.n_mels = corpus.channels, params.n_mels
+        self.stride = int(L.clx_batch_packed_stride(h))  # T_f
+        B, view = self.max_excerpts, self._batch.tensor
+        self.out = view(L.clx_batch_device_out(h), (self.channels, self.n_mels, self.stride), "<f4")
+        self._starts = view(L.clx_batch_packed_starts(h), (B,), "<i8")
+        self._frames = view(L.clx_batch_mel_frames(h), (B,), "<i8")
+        self._lengths = view(L.clx_batch_crop_lengths(h), (B,), "<i8")
+        self._status = view(L.clx_batch_crop_status(h), (B,), "<i4")
+        self._requests = view(L.clx_batch_packed_requests(h), (B, 3), "<i8")
+        self._count = view(L.clx_batch_packed_count(h), (1,), "<i4")
+        self._error = view(L.clx_batch_crop_error(h), (1,), "<i8")
+        self._stream = torch.cuda.ExternalStream(L.clx_ctx_stream(self.ctx._h, 0))
+        self._n = 0
+
+    def __call__(self, files, offsets=None, lengths=None, check: bool = True):
+        """Computes the features of excerpt b = samples [offsets[b], offsets[b] + lengths[b]) of file files[b], cut at
+        the file's end, for each of the n <= max_excerpts files, as PackedBatch.__call__ decodes them.  Returns
+        (features [C, n_mels, T_f], starts [n], frames [n], lengths [n]): frame starts and counts, lengths in samples."""
+        out, starts, lengths = super().__call__(files, offsets, lengths, check)
+        return out, starts, self._frames[:self._n], lengths
+
+    def _sample_start(self, b: int) -> int:
+        """Excerpt b's first sample column in the packed batch, for the first excerpt the error word reports: the ones
+        before it are valid and fit, so it is the sum of their round_up_4(length) (one sync)."""
+        return int(((self._lengths[:b] + 3) // 4 * 4).sum().item())

@@ -139,6 +139,9 @@ SYMBOLS = {
     "clx_batch_create_resampled_packed": (C.c_int, [_vp, _vp, _vp, _sz, _sz, _sz, C.c_uint32, C.POINTER(_vp)]),
     "clx_resample_packed_source_bound": (_sz, [_vp, _sz, C.c_uint32, _sz, _sz]),
     "clx_batch_create_mel_crops": (C.c_int, [_vp, _vp, _vp, _sz, _sz, _sz, C.c_uint32, _vp, _vp, _vp, C.POINTER(_vp)]),
+    "clx_batch_create_mel_packed": (C.c_int, [_vp, _vp, _vp, _sz, _sz, _sz, C.c_uint32, _vp, _vp, _vp, C.POINTER(_vp)]),
+    "clx_mel_packed_frames_bound": (_sz, [_vp, _sz, _sz]),
+    "clx_batch_mel_frames": (_vp, [_vp]),
     "clx_batch_decode": (C.c_int, [_vp, _vp, C.c_uint32]),
     "clx_batch_sync": (C.c_int, [_vp, _vp]),
     "clx_batch_read": (C.c_int, [_vp, _vp, _vp, _sz, _vp]),

@@ -23,6 +23,7 @@
 
 #include "claxon_b200.h"
 #include "clx_internal.h"
+#include "clx_mel.h"
 
 // A few long-lived host threads for the frame CRC-16 pass of batch creation from host bytes (precompute_crc):
 // spawning std::threads per batch costs more than the checksums themselves (6 MB per C2 batch).
@@ -243,10 +244,13 @@ struct clx_batch {
     clx_batch* inner = nullptr;
     clx::ResampleBuffers rs{};
     // Mel crop batches (clx_batch_create_mel_crops): `inner` is a crop or resampled crop batch, run before mel_kernel.
-    // crop.requests, status, lengths and error are the inner batch's; buf.conv is the features; mel the rest.
+    // crop.requests, status, lengths and error are the inner batch's; buf.conv is the features; mel the rest.  Mel
+    // packed batches (clx_batch_create_mel_packed) are those with `packed` set too: `inner` is a packed or resampled
+    // packed batch, packed.requests and count are its own, packed.starts the frame starts, and mel_packed the rest.
     bool is_mel = false;
     clx::MelBuffers mel{};
     size_t mel_smem = 0;
+    clx::MelPacked mel_packed{};
 };
 
 struct clx_corpus {
@@ -694,7 +698,9 @@ cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
     const clx::DecodeBuffers db = b->buf.view(b->n_frames, b->mode, b->stride);
     if (b->is_mel) {
         cudaError_t e = launch_batch(b->inner, st, launches);
-        if (e == cudaSuccess) e = clx::launch_mel(b->mel, b->mel_smem, st, launches);
+        if (e == cudaSuccess)
+            e = b->is_packed ? clx::launch_mel_packed(b->mel, b->mel_packed, b->mel_smem, st, launches)
+                             : clx::launch_mel(b->mel, b->mel_smem, st, launches);
         return e;
     }
     if (b->inner && b->is_packed) {
@@ -842,8 +848,10 @@ void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
     if (b->is_mel) {
         b->crop.requests = nullptr;  // the inner batch's, as status and error below
         b->crop.lengths = nullptr;
+        b->packed.requests = nullptr;
+        b->packed.count = nullptr;
         cudaFree((void*)b->mel.tw); cudaFree((void*)b->mel.window); cudaFree((void*)b->mel.bands);
-        cudaFree((void*)b->mel.weights);
+        cudaFree((void*)b->mel.weights); cudaFree(b->mel_packed.frames);
     }
     if (b->inner) {
         b->crop.status = nullptr;  // the inner batch's
@@ -1456,10 +1464,12 @@ int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t*
     *out = nullptr;
     if (!ctx || !corpus || n_crops == 0 || n_crops >= (1u << 30)) return CLX_ERR_INVALID_ARGUMENT;
     clx::MelTables t;
-    if (!clx::mel_tables(params, window, fbank, num_frames, &t)) return CLX_ERR_INVALID_ARGUMENT;
+    if (!clx::mel_tables(params, window, fbank, &t)) return CLX_ERR_INVALID_ARGUMENT;
+    const uint64_t F = clx::mel_frame_count(num_frames, params->n_fft, params->hop_length, params->flags & CLX_MEL_CENTER);
+    if (F == 0) return CLX_ERR_INVALID_ARGUMENT;  // a row too short for a frame, or for the reflect pad
     const size_t C = corpus->channels, rows = n_crops * C;  // (< 2^33: no overflow)
-    const uint64_t tiles = (t.F + t.tile - 1) / t.tile;
-    if (t.F > (SIZE_MAX / 4 - 8) / (rows * params->n_mels) || tiles >= (1u << 31) / rows) return CLX_ERR_INVALID_ARGUMENT;
+    const uint64_t tiles = (F + t.tile - 1) / t.tile;
+    if (F > (SIZE_MAX / 4 - 8) / (rows * params->n_mels) || tiles >= (1u << 31) / rows) return CLX_ERR_INVALID_ARGUMENT;
     clx_batch* inner = nullptr;
     const int rc = target_rate ? clx_batch_create_resampled_crops(ctx, corpus, file_rates, n_files, n_crops, num_frames,
                                                                   target_rate, &inner)
@@ -1470,9 +1480,9 @@ int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t*
     corpus->live++;
     b->inner = inner;
     b->is_mel = true;
-    b->out_elems = rows * params->n_mels * t.F;
+    b->out_elems = rows * params->n_mels * F;
     b->mode = CLX_OUT_CHANNELS_F32;
-    b->stride = t.F;
+    b->stride = F;
     b->crop.requests = inner->crop.requests;
     b->crop.status = inner->crop.status;
     b->crop.lengths = inner->crop.lengths;
@@ -1483,7 +1493,7 @@ int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t*
     clx::MelBuffers& mb = b->mel;
     mb.src = reinterpret_cast<const float*>(inner->buf.conv);
     mb.L = num_frames;
-    mb.F = t.F;
+    mb.F = F;
     mb.rows = (uint32_t)rows;
     mb.tiles = (uint32_t)tiles;
     mb.n_fft = params->n_fft;
@@ -1512,6 +1522,87 @@ int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t*
     *out = b;
     return CLX_OK;
 }
+
+int clx_batch_create_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                                size_t max_excerpts, size_t max_samples, uint32_t target_rate,
+                                const clx_mel_params* params, const float* window, const float* fbank,
+                                clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (!ctx || !corpus || max_excerpts == 0 || max_excerpts >= (1u << 30) || max_samples == 0)
+        return CLX_ERR_INVALID_ARGUMENT;
+    clx::MelTables t;
+    if (!clx::mel_tables(params, window, fbank, &t)) return CLX_ERR_INVALID_ARGUMENT;
+    const size_t F = clx::mel_packed_frames(params, max_excerpts, max_samples), C = corpus->channels;
+    const uint64_t tiles = std::max<uint64_t>(1, (F + t.tile - 1) / t.tile);  // (one CTA per row when F is 0)
+    if (F == SIZE_MAX || F > (SIZE_MAX / 4 - 8) / (C * params->n_mels) || tiles >= (1u << 31) / C)
+        return CLX_ERR_INVALID_ARGUMENT;
+    clx_batch* inner = nullptr;
+    const int rc = target_rate ? clx_batch_create_resampled_packed(ctx, corpus, file_rates, n_files, max_excerpts,
+                                                                   max_samples, target_rate, &inner)
+                               : clx_batch_create_packed(ctx, corpus, max_excerpts, max_samples, CLX_OUT_CHANNELS_F32,
+                                                         &inner);
+    if (rc != CLX_OK) return rc;
+    clx_batch* b = new clx_batch();
+    b->corpus = corpus;
+    corpus->live++;
+    b->inner = inner;
+    b->is_mel = true;
+    b->is_packed = true;
+    b->out_elems = C * params->n_mels * F;
+    b->mode = CLX_OUT_CHANNELS_F32;
+    b->stride = F;
+    b->crop.requests = inner->crop.requests;
+    b->crop.status = inner->crop.status;
+    b->crop.lengths = inner->crop.lengths;
+    b->crop.error = inner->crop.error;
+    b->crop.n_crops = (uint32_t)max_excerpts;
+    b->crop.C = (uint32_t)C;
+    b->packed.requests = inner->packed.requests;
+    b->packed.count = inner->packed.count;
+    b->packed.T = max_samples;
+    clx::MelBuffers& mb = b->mel;
+    mb.src = reinterpret_cast<const float*>(inner->buf.conv);
+    mb.L = inner->stride;
+    mb.F = F;
+    mb.rows = (uint32_t)C;
+    mb.tiles = (uint32_t)tiles;
+    mb.n_fft = params->n_fft;
+    mb.hop = params->hop_length;
+    mb.n_mels = params->n_mels;
+    mb.tile = t.tile;
+    mb.flags = params->flags;
+    mb.log_floor = params->log_floor;
+    mb.log_of_floor = (params->flags & CLX_MEL_LOG) ? (float)std::log((double)params->log_floor) : 0.f;
+    b->mel_smem = t.smem;
+    clx::MelPacked& mp = b->mel_packed;
+    mp.count = inner->packed.count;
+    mp.lengths = inner->crop.lengths;
+    mp.src_starts = inner->packed.starts;
+    mp.n = (uint32_t)max_excerpts;
+    cudaError_t e = cudaSetDevice(ctx->device);
+    if (e == cudaSuccess) e = clx::mel_init();
+    if (e == cudaSuccess) e = device_zeros(b->buf.conv, (b->out_elems + 8) * sizeof(float));  // (the slack of fit())
+    if (e == cudaSuccess) e = device_zeros(b->packed.starts, max_excerpts);
+    if (e == cudaSuccess) e = device_zeros(mp.frames, max_excerpts);
+    if (e == cudaSuccess) e = upload(mb.tw, t.tw);
+    if (e == cudaSuccess) e = upload(mb.window, t.window);
+    if (e == cudaSuccess) e = upload(mb.bands, t.bands);
+    if (e == cudaSuccess) e = upload(mb.weights, t.weights);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
+    if (e != cudaSuccess) {
+        clx_batch_destroy(ctx, b);
+        return cuda_fail(ctx, e, "clx_batch_create_mel_packed");
+    }
+    mp.starts = b->packed.starts;
+    mb.out = reinterpret_cast<float*>(b->buf.conv);
+    build_graph(ctx, b);
+    *out = b;
+    return CLX_OK;
+}
+
+void* clx_batch_mel_frames(clx_batch* b) { return b && b->is_mel && b->is_packed ? (void*)b->mel_packed.frames : nullptr; }
 
 }  // extern "C"
 

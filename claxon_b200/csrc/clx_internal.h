@@ -245,18 +245,35 @@ struct MelBuffers {
     uint32_t flags;         // CLX_MEL_*
     float log_floor, log_of_floor;  // ln(log_floor), taken in float64
 };
-// The host side of clx_batch_create_mel_crops: the checks of the header's refusals that do not depend on the inner
-// batch, the frame count F and the tables.  false for a refusal.
+// The host side of clx_batch_create_mel_crops and _mel_packed: the checks of the header's refusals that depend neither
+// on the inner batch nor on a row length, and the tables.  false for a refusal.  mel_params_ok: those checks of the
+// parameters alone (params not NULL included).
 struct MelTables {
     std::vector<float> tw, window, weights;
     std::vector<MelBand> bands;
-    uint64_t F = 0;
     uint32_t tile = 0;
     size_t smem = 0;
 };
-bool mel_tables(const clx_mel_params* p, const float* window, const float* fbank, size_t num_frames, MelTables* t);
-cudaError_t mel_init();  // mel_kernel's shared memory limit, on the current device, before a graph captures it
+bool mel_params_ok(const clx_mel_params* p);
+bool mel_tables(const clx_mel_params* p, const float* window, const float* fbank, MelTables* t);
+cudaError_t mel_init();  // the mel kernels' shared memory limit, on the current device, before a graph captures them
 cudaError_t launch_mel(const MelBuffers& mb, size_t smem, cudaStream_t stream, uint64_t* launches);
+// Mel packed batches (clx_batch_create_mel_packed) keep a MelBuffers with src = the inner packed batch's [C, L] output
+// (L its row stride), rows = C, F = the frame columns T_f (the features' row pitch), and this: the inner batch's count,
+// lengths in samples and sample starts, and the batch's own frame starts and frame counts, written by the planner.
+struct MelPacked {
+    const uint32_t* count;
+    const int64_t* lengths;
+    const int64_t* src_starts;
+    int64_t* starts;
+    int64_t* frames;
+    uint32_t n;  // max_excerpts
+};
+// clx_mel_packed_frames_bound of valid parameters: SIZE_MAX if it overflows.
+size_t mel_packed_frames(const clx_mel_params* p, size_t max_excerpts, size_t max_samples);
+// The planner (frame counts and starts) and mel_packed_kernel, after the inner batch's launch sequence.
+cudaError_t launch_mel_packed(const MelBuffers& mb, const MelPacked& mp, size_t smem, cudaStream_t stream,
+                              uint64_t* launches);
 #ifdef CLX_EXPERIMENT
 extern int g_exp_which;  // measurement builds only: bit 0 = index pass, bit 1 = decode pass of LanePerFrame
 extern int g_exp_dyn_smem;

@@ -7,6 +7,11 @@
 // frame's power |X[k]|^2, k <= n_fft / 2, into the free buffer; then each thread sums one (mel, frame) over the mel's
 // non-zero bins, threads laid along the frames so that each mel row of the tile is stored contiguously.  Every sum has
 // one fixed order and no atomics: calls are bit-identical.
+//
+// Mel packed batches (clx_batch_create_mel_packed) run two kernels after an inner packed or resampled packed batch:
+// mel_packed_plan_kernel gives each excerpt its frame count and frame start, and mel_packed_kernel computes the frames
+// of one (tile of frame columns, row) per CTA with mel_kernel's per-frame arithmetic, once over the whole tile whatever
+// the excerpts in it.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -16,6 +21,7 @@
 #include "claxon_b200.h"
 #include "clx_internal.h"
 #include "clx_mel.h"
+#include "clx_scan.cuh"
 
 namespace clx {
 
@@ -102,12 +108,167 @@ mel_kernel(MelBuffers mb) {
     }
 }
 
+// One CTA, SCAN_THREADS excerpts at a time: F_b = mel_frame_count(n_b) of the inner batch's length n_b (0 for an
+// invalid, non-fitting or empty excerpt), start_0 = 0 and start_{b+1} = start_b + round_up_4(F_b), for b < count.
+__global__ void __launch_bounds__(SCAN_THREADS)
+mel_packed_plan_kernel(MelPacked mp, uint32_t n_fft, uint32_t hop, bool center) {
+    __shared__ PackedSums s_warp[SCAN_THREADS / 32];
+    __shared__ PackedSums s_cols;
+    if (threadIdx.x == 0) s_cols = PackedSums{};
+    __syncthreads();
+    const uint32_t used = min(*mp.count, mp.n);
+    for (uint32_t base = 0; base < used; base += SCAN_THREADS) {
+        const uint32_t b = base + threadIdx.x;
+        const uint64_t F = b < used ? mel_frame_count((uint64_t)mp.lengths[b], n_fft, hop, center) : 0;
+        const uint64_t start = cta_scan(PackedSums{(F + 3) & ~(uint64_t)3, 0, 0, 0}, s_warp, &s_cols).cols;
+        if (b < used) {
+            mp.starts[b] = (int64_t)start;
+            mp.frames[b] = (int64_t)F;
+        }
+    }
+}
+
+// Frame j of an excerpt whose n samples start at column base of the inner output's rows.
+struct MelSlot {
+    int64_t base, n;
+    uint32_t j;
+};
+
+// mel_kernel over frame columns [t0, t0 + nf) of features row `row` of the packed layout.  Each of the tile's columns
+// finds its excerpt by binary search (the ends start_b + F_b never decrease, since start_{b+1} >= start_b + F_b): the
+// first b whose end passes the column holds it if start_b <= the column, else the column is an alignment gap or lies
+// past the last excerpt.  The tile's frames are compacted into slots 0 .. nv - 1, the one windowing, FFT and power pass
+// runs over those, and each column stores its slot's mel sums, or 0 for a column without a frame.
+__global__ void __launch_bounds__(MEL_THREADS)
+mel_packed_kernel(MelBuffers mb, MelPacked mp) {
+    extern __shared__ MelCpx s_buf[];  // two buffers of tile * N points
+    __shared__ MelSlot s_slot[MEL_MAX_TILE];
+    __shared__ int32_t s_col[MEL_MAX_TILE];  // column f's slot, -1 for none
+    __shared__ uint32_t s_nv;
+    const uint32_t N = mb.n_fft / 2, T = mb.tile;
+    const uint32_t row = blockIdx.x / mb.tiles, tile = blockIdx.x - row * mb.tiles;
+    const uint64_t t0 = (uint64_t)tile * T;
+    const uint32_t nf = (uint32_t)min((uint64_t)T, mb.F - t0);
+    if (threadIdx.x < 32) {  // T <= 32: one warp
+        const uint32_t f = threadIdx.x, used = min(*mp.count, mp.n);
+        const uint64_t t = t0 + f;
+        bool valid = false;
+        MelSlot s{0, 0, 0};
+        if (f < nf) {
+            uint32_t lo = 0, hi = used;
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if ((uint64_t)(mp.starts[mid] + mp.frames[mid]) > t) hi = mid;
+                else lo = mid + 1;
+            }
+            if (lo < used && (uint64_t)mp.starts[lo] <= t) {
+                valid = true;
+                s = MelSlot{mp.src_starts[lo], mp.lengths[lo], (uint32_t)(t - (uint64_t)mp.starts[lo])};
+            }
+        }
+        const uint32_t mask = __ballot_sync(0xffffffffu, valid), slot = __popc(mask & ((1u << f) - 1));
+        if (valid) s_slot[slot] = s;
+        if (f < T) s_col[f] = valid ? (int32_t)slot : -1;
+        if (f == 0) s_nv = __popc(mask);
+    }
+    __syncthreads();
+    const uint32_t nv = s_nv;
+    const MelCpx* tw = reinterpret_cast<const MelCpx*>(mb.tw);
+    MelCpx* a = s_buf;
+    MelCpx* b = s_buf + T * N;
+    const uint32_t K = N + 1, P = K | 1;
+    float* pw = reinterpret_cast<float*>(b);
+    if (nv) {
+        // 1. The frames, windowed, as in mel_kernel, each reflect-padded within its own excerpt (n > N with
+        //    CLX_MEL_CENTER, n >= n_fft without: every index reflects into the excerpt once, or not at all).
+        const int64_t pad = (mb.flags & CLX_MEL_CENTER) ? (int64_t)N : 0;
+        const float* xr = mb.src + (uint64_t)row * mb.L;
+        {
+            const uint32_t df = MEL_THREADS / N, dq = MEL_THREADS - df * N;
+            for (uint32_t f = threadIdx.x / N, q = threadIdx.x - f * N; f < nv;) {
+                const MelSlot s = s_slot[f];
+                const float* x = xr + s.base;
+                const int64_t p = (int64_t)s.j * mb.hop + 2 * q - pad, L = s.n;
+                float v[2];
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    int64_t i = p + h;
+                    i = i < 0 ? -i : i >= L ? 2 * L - 2 - i : i;
+                    const float w = __ldg(mb.window + 2 * q + h);
+                    v[h] = w != 0.f ? w * __ldg(x + i) : 0.f;
+                }
+                a[f * N + q] = MelCpx{v[0], v[1]};
+                q += dq;
+                f += df;
+                if (q >= N) {
+                    q -= N;
+                    f++;
+                }
+            }
+        }
+        // 2. The FFT of every slot.
+        for (uint32_t Ns = 1, R; Ns < N; Ns *= R) {
+            R = mel_radix(N / Ns);
+            __syncthreads();
+            mel_stage(a, b, tw, N, Ns, R, nv, threadIdx.x, MEL_THREADS);
+            MelCpx* t = a;
+            a = b;
+            b = t;
+        }
+        __syncthreads();
+        // 3. The power of bins 0 .. N of slot f at pw[f * P + k].
+        pw = reinterpret_cast<float*>(b);
+        const uint32_t df = MEL_THREADS / K, dk = MEL_THREADS - df * K;
+        for (uint32_t f = threadIdx.x / K, k = threadIdx.x - f * K; f < nv;) {
+            pw[f * P + k] = mel_power(a + f * N, tw, N, k);
+            k += dk;
+            f += df;
+            if (k >= K) {
+                k -= K;
+                f++;
+            }
+        }
+        __syncthreads();
+    }
+    // 4. The mel sums of every column of the tile, frames fastest; 0 where a column has no frame.
+    const bool log = mb.flags & CLX_MEL_LOG;
+    const uint32_t shift = __ffs(T) - 1;
+    for (uint32_t i = threadIdx.x; i < mb.n_mels * T; i += MEL_THREADS) {
+        const uint32_t m = i >> shift, f = i & (T - 1);
+        if (f >= nf) continue;
+        const int32_t sl = s_col[f];
+        float acc = 0.f;
+        if (sl >= 0) {
+            const MelBand band = mb.bands[m];
+            const float* w = mb.weights + band.w;
+            const float* s = pw + (uint32_t)sl * P + band.lo;
+            for (uint32_t k = 0; k < band.n; k++) acc = fmaf(__ldg(w + k), s[k], acc);
+            if (log) acc = acc > mb.log_floor ? logf(acc) : mb.log_of_floor;
+        }
+        mb.out[((uint64_t)row * mb.n_mels + m) * mb.F + t0 + f] = acc;
+    }
+}
+
 cudaError_t mel_init() {  // the most any batch uses, so that no batch lowers another's limit
-    return cudaFuncSetAttribute(mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MEL_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MEL_SMEM);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(mel_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MEL_SMEM);
+    return e;
 }
 
 cudaError_t launch_mel(const MelBuffers& mb, size_t smem, cudaStream_t stream, uint64_t* launches) {
     mel_kernel<<<mb.rows * mb.tiles, MEL_THREADS, smem, stream>>>(mb);
+    (*launches)++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_mel_packed(const MelBuffers& mb, const MelPacked& mp, size_t smem, cudaStream_t stream,
+                              uint64_t* launches) {
+    mel_packed_plan_kernel<<<1, SCAN_THREADS, 0, stream>>>(mp, mb.n_fft, mb.hop, (mb.flags & CLX_MEL_CENTER) != 0);
+    (*launches)++;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    mel_packed_kernel<<<mb.rows * mb.tiles, MEL_THREADS, smem, stream>>>(mb, mp);
     (*launches)++;
     return cudaGetLastError();
 }
@@ -123,16 +284,18 @@ bool smooth(uint32_t n) {  // no prime factor above 5
 }
 }  // namespace
 
-bool mel_tables(const clx_mel_params* p, const float* window, const float* fbank, size_t num_frames, MelTables* t) {
-    if (!p || !window || !fbank) return false;
-    const uint32_t n_fft = p->n_fft, N = n_fft / 2;
-    if (n_fft % 2 || n_fft < 8 || n_fft > 4096 || !smooth(N) || p->win_length < 1 || p->win_length > n_fft ||
+bool mel_params_ok(const clx_mel_params* p) {
+    if (!p) return false;
+    const uint32_t n_fft = p->n_fft;
+    if (n_fft % 2 || n_fft < 8 || n_fft > 4096 || !smooth(n_fft / 2) || p->win_length < 1 || p->win_length > n_fft ||
         p->hop_length < 1 || p->n_mels < 1 || p->n_mels > 512 || (p->flags & ~(CLX_MEL_CENTER | CLX_MEL_LOG)))
         return false;
-    if ((p->flags & CLX_MEL_LOG) ? !(std::isfinite(p->log_floor) && p->log_floor > 0.f) : p->log_floor != 0.f)
-        return false;
-    if ((p->flags & CLX_MEL_CENTER) ? num_frames <= N : num_frames < n_fft) return false;
-    t->F = (p->flags & CLX_MEL_CENTER) ? 1 + num_frames / p->hop_length : 1 + (num_frames - n_fft) / p->hop_length;
+    return (p->flags & CLX_MEL_LOG) ? std::isfinite(p->log_floor) && p->log_floor > 0.f : p->log_floor == 0.f;
+}
+
+bool mel_tables(const clx_mel_params* p, const float* window, const float* fbank, MelTables* t) {
+    if (!mel_params_ok(p) || !window || !fbank) return false;
+    const uint32_t n_fft = p->n_fft, N = n_fft / 2;
     t->window.assign(n_fft, 0.f);
     const uint32_t w0 = (n_fft - p->win_length) / 2;
     for (uint32_t i = 0; i < p->win_length; i++) {
@@ -170,4 +333,23 @@ bool mel_tables(const clx_mel_params* p, const float* window, const float* fbank
     return true;
 }
 
+// The frame columns of the excerpts that fit in a packed batch of B excerpts and T sample columns (DESIGN §3.6).  The
+// excerpts with frames have n_b >= m, m the shortest row with a frame (n_fft / 2 + 1 with CLX_MEL_CENTER, n_fft
+// without); all but the last of them take round_up_4(n_b) >= round_up_4(m) columns before the last one's start, and
+// that one ends by T: k <= min(B, (T - m) / round_up_4(m) + 1) of them, and the n_b add up to T at most.  Each takes
+// round_up_4(F_b) <= F_b + 3 <= n_b / hop + 4 frame columns, and the floors of n_b / hop add up to floor(T / hop) at
+// most: round_up_4(floor(T / hop) + 4k) in all.
+size_t mel_packed_frames(const clx_mel_params* p, size_t max_excerpts, size_t max_samples) {
+    const uint64_t m = (p->flags & CLX_MEL_CENTER) ? p->n_fft / 2 + 1 : p->n_fft, m4 = (m + 3) & ~(uint64_t)3;
+    if (max_samples < m) return 0;
+    const uint64_t k = std::min<uint64_t>(max_excerpts, (max_samples - m) / m4 + 1);
+    const unsigned __int128 cols = (unsigned __int128)(max_samples / p->hop_length) + 4 * (unsigned __int128)k + 3;
+    return cols > SIZE_MAX ? SIZE_MAX : (size_t)(cols & ~(unsigned __int128)3);
+}
+
 }  // namespace clx
+
+extern "C" size_t clx_mel_packed_frames_bound(const clx_mel_params* params, size_t max_excerpts, size_t max_samples) {
+    if (!clx::mel_params_ok(params) || max_excerpts == 0 || max_samples == 0) return 0;
+    return clx::mel_packed_frames(params, max_excerpts, max_samples);
+}

@@ -1,4 +1,4 @@
-// clx_mel.h — the per-frame arithmetic of mel_kernel (clx_mel.cu): the real FFT of n_fft = 2N samples as a complex
+// clx_mel.h — the per-frame arithmetic of mel_kernel and mel_packed_kernel (clx_mel.cu): the real FFT of n_fft = 2N samples as a complex
 // Stockham FFT of N points (radices 4, 2, 3, 5) and the even / odd split to |X[k]|^2, k <= N.  Plain C++ as well as
 // CUDA, so that tools/mel_host.cpp runs the very code the kernel runs on the host (tests/test_mel_host.py).
 #ifndef CLX_MEL_H
@@ -18,6 +18,13 @@ struct alignas(8) MelCpx {
 };
 
 CLX_MEL_HD MelCpx mel_mul(MelCpx a, MelCpx b) { return {a.re * b.re - a.im * b.im, a.re * b.im + a.im * b.re}; }
+
+// The frames of a row of n samples: 1 + n / hop reflect-padded (n > n_fft / 2, the pad torch.stft accepts), else
+// 1 + (n - n_fft) / hop (n >= n_fft); 0 for a shorter row.
+CLX_MEL_HD uint64_t mel_frame_count(uint64_t n, uint32_t n_fft, uint32_t hop, bool center) {
+    if (center) return n > n_fft / 2 ? 1 + n / hop : 0;
+    return n >= n_fft ? 1 + (n - n_fft) / hop : 0;
+}
 
 // The radix of the Stockham stage that has `left` = N / Ns points still to combine.
 CLX_MEL_HD uint32_t mel_radix(uint32_t left) { return left % 4 == 0 ? 4 : left % 2 == 0 ? 2 : left % 3 == 0 ? 3 : 5; }

@@ -558,6 +558,43 @@ int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t*
                                size_t n_crops, size_t num_frames, uint32_t target_rate, const clx_mel_params* params,
                                const float* window /* win_length */, const float* fbank /* [n_fft / 2 + 1][n_mels] */,
                                clx_batch** out);
+/* Mel packed batches: the mel spectrogram of every excerpt of a packed batch, packed along frames.  The inner batch is
+ * clx_batch_create_packed(ctx, corpus, max_excerpts, max_samples, CLX_OUT_CHANNELS_F32) when target_rate is 0 (file_rates
+ * may then be NULL), else clx_batch_create_resampled_packed(ctx, corpus, file_rates, n_files, max_excerpts, max_samples,
+ * target_rate); x is its [C, stride] output, s_b and n_b excerpt b's sample start and length.  Excerpt b's frames are
+ * clx_batch_create_mel_crops's transform of the row slices x[:, s_b : s_b + n_b], each reflect-padded with its own
+ * samples at its own two edges, with the same params, window and fbank: F_b = 1 + n_b / hop_length when n_b > n_fft / 2
+ * with CLX_MEL_CENTER, 1 + (n_b - n_fft) / hop_length when n_b >= n_fft without, else 0.  So an invalid, non-fitting,
+ * empty or unused excerpt (n_b = 0) has no frames, and so has one too short for a frame: its status and length stay the
+ * inner batch's.  Rows its file does not have are zeros in x and are transformed like the others (exactly 0, or
+ * ln(log_floor) with CLX_MEL_LOG).  Layout: start_0 = 0, start_{b+1} = start_b + round_up_4(F_b); the output is [C,
+ * n_mels, T_f] float32, T_f = clx_mel_packed_frames_bound(params, max_excerpts, max_samples), element (c, m, t) at (c *
+ * n_mels + m) * T_f + t, and excerpt b's frames are columns [start_b, start_b + F_b).  Every other element reads 0 after
+ * every call, with or without the log: alignment gaps and every column past the call's last excerpt.  T_f holds the
+ * frames of any excerpts that fit the inner batch, so the fit rule is the packed batch's alone.  Each call is the inner
+ * batch's launch sequence and two kernels: one CTA that counts and lays out the frames (device memory, written by each
+ * call for b < count: clx_batch_mel_frames, int64 F_b; clx_batch_packed_starts, int64 start_b), and one CTA per (tile of
+ * frame columns, row) that runs the windowing, FFT, power and mel sums of clx_batch_create_mel_crops once per tile,
+ * whatever the excerpts it spans.  No atomics: calls are bit-identical.  Accessors: clx_batch_packed_requests and _count
+ * are the inner batch's (requests at the inner batch's rate); clx_batch_crop_status, _lengths (samples) and _error are
+ * the inner batch's; clx_batch_packed_stride is T_f; clx_batch_device_out the features.  Memory: the inner batch, C *
+ * n_mels * T_f floats, 16 bytes per excerpt and tables of a few times n_fft floats.
+ * CLX_ERR_INVALID_ARGUMENT for what the inner create refuses; every parameter clx_batch_create_mel_crops refuses (NULL
+ * params, window or fbank, n_fft, win_length, hop_length, n_mels, flags, log_floor, non-finite window or fbank values);
+ * max_excerpts 0 or 2^30 or more, max_samples 0; sizes that overflow.  No length is refused: a too short excerpt has 0
+ * frames. */
+int clx_batch_create_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                                size_t max_excerpts, size_t max_samples, uint32_t target_rate,
+                                const clx_mel_params* params, const float* window /* win_length */,
+                                const float* fbank /* [n_fft / 2 + 1][n_mels] */, clx_batch** out);
+/* The frame columns T_f of a mel packed batch: at least sum_b round_up_4(F_b) over any excerpts that fit in max_samples
+ * (T) columns of max_excerpts (B), a multiple of 4.  With m the shortest length that has a frame (n_fft / 2 + 1 with
+ * CLX_MEL_CENTER, n_fft without) and k = min(B, (T - m) / round_up_4(m) + 1) the most excerpts with frames that fit:
+ * round_up_4(floor(T / hop_length) + 4k), and 0 when T < m.  SIZE_MAX if that overflows.  0 also for params that
+ * clx_batch_create_mel_crops refuses, or a zero argument.  Host only; no context. */
+size_t clx_mel_packed_frames_bound(const clx_mel_params* params, size_t max_excerpts, size_t max_samples);
+/* Device pointer of a mel packed batch's max_excerpts int64 frame counts F_b (NULL for other batches). */
+void* clx_batch_mel_frames(clx_batch* b);
 int clx_batch_decode(clx_ctx* ctx, clx_batch* b, uint32_t stream_index); /* async on an internal stream */
 int clx_batch_sync(clx_ctx* ctx, clx_batch* b);
 /* Planar batches only (CLX_ERR_INVALID_ARGUMENT for any other mode). */

@@ -1091,9 +1091,12 @@ class Corpus:
     def resample_packed_source_bound(self, max_excerpts: int, max_samples: int, sample_rate: int) -> int:
         """clx_resample_packed_source_bound: the columns of the packed batch that decodes the source spans of a
         resampled PackedBatch (about max_samples x r / R for the corpus's highest rate r)."""
-        rates = np.array([f.info.sample_rate for f in self.index.files] or [0], dtype=np.uint32)
-        return int(self.ctx._L.clx_resample_packed_source_bound(rates.ctypes.data, len(self.index), int(sample_rate),
-                                                                int(max_excerpts), int(max_samples)))
+        return int(self.ctx._L.clx_resample_packed_source_bound(self._file_rates().ctypes.data, len(self.index),
+                                                                int(sample_rate), int(max_excerpts), int(max_samples)))
+
+    def _file_rates(self) -> np.ndarray:
+        """Each file's STREAMINFO sample rate, uint32 (one 0 for a corpus without files, so that it has an address)."""
+        return np.array([f.info.sample_rate for f in self.index.files] or [0], dtype=np.uint32)
 
     @classmethod
     def share(cls, index: FlacIndex, path, ctx: Context | None = None) -> "Corpus":
@@ -1260,6 +1263,24 @@ class Corpus:
 _still_registered = []
 
 
+def _first_failure(error) -> tuple[int, int, int] | None:
+    """The error word of a crop or packed batch, read with the call's one sync: None, or the first failed excerpt's
+    (kind, index, status), kind 0 being an invalid or non-fitting request."""
+    err = int(error.item()) & ((1 << 64) - 1)
+    if err == (1 << 64) - 1:
+        return None
+    st = err & 0xffffffff
+    return err >> 62, (err >> 32) & ((1 << 30) - 1), st - (1 << 32) if st >= 1 << 31 else st
+
+
+def _length_at(f: IndexedFile, rate: int | None) -> tuple[int, str]:
+    """File f's length in samples at `rate`, ceil(N * R / r), and " at R Hz"; N and "" at its own rate or None."""
+    if rate is None or f.info.sample_rate == rate:
+        return f.length, ""
+    g = math.gcd(f.info.sample_rate, rate)
+    return -(-f.length * (rate // g) // (f.info.sample_rate // g)), f" at {rate} Hz"
+
+
 class CropBatch:
     """`batch` excerpts of `num_frames` samples of a Corpus's files per call, as one [B, C, L] CUDA tensor
     (clx_batch_create_crops): the crops' frames, windows and columns are planned on the device inside the batch's CUDA
@@ -1288,28 +1309,30 @@ class CropBatch:
     the device."""
 
     def __init__(self, corpus: Corpus, batch: int, num_frames: int, dtype=None, sample_rate: int | None = None):
-        import torch
-        dtype = _torch_dtype(dtype)
-        self.corpus, self.ctx = corpus, corpus.ctx
-        self.batch, self.num_frames, self.dtype = int(batch), int(num_frames), dtype
-        self.sample_rate = None if sample_rate is None else int(sample_rate)
-        if self.batch < 1 or self.num_frames < 1:
-            raise ValueError("batch and num_frames must be >= 1")
-        mode = _channels_mode(dtype)
+        mode = self._args(corpus, batch, num_frames, dtype, sample_rate)
         L = self.ctx._L
         h = C.c_void_p()
         if self.sample_rate is None:
             _check(L.clx_batch_create_crops(self.ctx._h, corpus._h, self.batch, self.num_frames, mode, C.byref(h)),
                    self.ctx)
         else:
-            if dtype != torch.float32:
-                raise ValueError("a resampled crop batch is float32 only")
-            rates = np.array([f.info.sample_rate for f in corpus.index.files] or [0], dtype=np.uint32)
-            _check(L.clx_batch_create_resampled_crops(self.ctx._h, corpus._h, rates.ctypes.data, len(corpus.index),
-                                                      self.batch, self.num_frames, self.sample_rate, C.byref(h)),
-                   self.ctx)
+            _check(L.clx_batch_create_resampled_crops(self.ctx._h, corpus._h, corpus._file_rates().ctypes.data,
+                                                      len(corpus.index), self.batch, self.num_frames, self.sample_rate,
+                                                      C.byref(h)), self.ctx)
         self.channels = corpus.channels
         self._attach(h, (self.batch, self.channels, self.num_frames), "<f4" if mode == OUT_CHANNELS_F32 else "<i4")
+
+    def _args(self, corpus: Corpus, batch: int, num_frames: int, dtype, sample_rate: int | None) -> int:
+        """Checks and keeps the arguments of every crop batch; returns the output mode."""
+        import torch
+        self.corpus, self.ctx = corpus, corpus.ctx
+        self.batch, self.num_frames, self.dtype = int(batch), int(num_frames), _torch_dtype(dtype)
+        self.sample_rate = None if sample_rate is None else int(sample_rate)
+        if self.batch < 1 or self.num_frames < 1:
+            raise ValueError("batch and num_frames must be >= 1")
+        if self.sample_rate is not None and self.dtype != torch.float32:
+            raise ValueError("a resampled crop batch is float32 only")
+        return _channels_mode(self.dtype)
 
     def _attach(self, h, out_shape: tuple, typestr: str):
         """Takes ownership of the created batch `h` and views its buffers: out, lengths, status, requests, error."""
@@ -1324,20 +1347,6 @@ class CropBatch:
         self._error = view(L.clx_batch_crop_error(h), (1,), "<i8")
         self._stream = torch.cuda.ExternalStream(L.clx_ctx_stream(self.ctx._h, 0))
 
-    def _column(self, x, what: str):
-        import torch
-        if isinstance(x, torch.Tensor):
-            if x.dtype.is_floating_point or x.dtype.is_complex or x.dtype == torch.bool:
-                raise TypeError(f"{what} must hold integers")
-            t = x.reshape(-1)
-        else:
-            t = torch.from_numpy(np.asarray(x, dtype=np.int64).reshape(-1))
-        if t.numel() != self.batch:
-            raise ValueError(f"{what}: {t.numel()} values for a batch of {self.batch}")
-        if not t.is_cuda:
-            t = t.to(torch.int64).pin_memory().to("cuda", non_blocking=True)
-        return t
-
     def __call__(self, files, offsets, check: bool = True):
         """Decodes crop b = samples [offsets[b], offsets[b] + L) of file files[b] for every b.  Returns (out [B, C, L],
         lengths [B] int64), both on the GPU.  The requests are copied on torch's current stream, the batch's stream
@@ -1348,7 +1357,8 @@ class CropBatch:
         check=False nothing is raised; `status` holds each crop's outcome (CLX_ERR_INVALID_ARGUMENT, 90, for a request
         out of range, whose rows are zero and length 0) and a failed crop's rows are unspecified."""
         import torch
-        files, offsets = self._column(files, "files"), self._column(offsets, "offsets")
+        files = _request_column(files, self.batch, "files", "a batch of {}")
+        offsets = _request_column(offsets, self.batch, "offsets", "a batch of {}")
         self._requests[:, 0].copy_(files)
         self._requests[:, 1].copy_(offsets)
         self._stream.wait_stream(torch.cuda.current_stream())
@@ -1359,21 +1369,16 @@ class CropBatch:
         return self.out, self.lengths
 
     def _raise(self):
-        err = int(self._error.item()) & ((1 << 64) - 1)  # the one sync
-        if err == (1 << 64) - 1:
+        failure = _first_failure(self._error)
+        if failure is None:
             return
-        kind, b, st = err >> 62, (err >> 32) & ((1 << 30) - 1), err & 0xffffffff
-        st = st - (1 << 32) if st >= 1 << 31 else st
+        kind, b, st = failure
         fi, o = (int(v) for v in self._requests[b].tolist())
         if kind == 0:
             if not 0 <= fi < len(self.corpus.index):
                 raise ValueError(f"crop {b}: file index {fi} out of range")
-            f = self.corpus.index[fi]
-            if self.sample_rate is None or f.info.sample_rate == self.sample_rate:
-                raise ValueError(f"crop {b}: offset {o} outside file {fi} ({f.length} samples)")
-            g = math.gcd(f.info.sample_rate, self.sample_rate)
-            Nt = -(-f.length * (self.sample_rate // g) // (f.info.sample_rate // g))
-            raise ValueError(f"crop {b}: offset {o} outside file {fi} ({Nt} samples at {self.sample_rate} Hz)")
+            N, at = _length_at(self.corpus.index[fi], self.sample_rate)
+            raise ValueError(f"crop {b}: offset {o} outside file {fi} ({N} samples{at})")
         raise Error(st, f"file {fi}, crop {b}")
 
     def kernel_ms(self) -> float:
@@ -1475,21 +1480,15 @@ class MelCropBatch(CropBatch):
                  n_fft: int = 400, win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
                  f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
                  center: bool = True, norm: str | None = None, mel_scale: str = "htk", log_floor: float | None = None):
-        import torch
-        self.corpus, self.ctx = corpus, corpus.ctx
-        self.batch, self.num_frames, self.dtype = int(batch), int(num_frames), torch.float32
-        self.sample_rate = None if sample_rate is None else int(sample_rate)
-        if self.batch < 1 or self.num_frames < 1:
-            raise ValueError("batch and num_frames must be >= 1")
+        self._args(corpus, batch, num_frames, None, sample_rate)
         params, window, fbank = _mel_tables(_mel_rate(corpus.index, self.sample_rate), n_fft, win_length, hop_length,
                                             f_min, f_max, n_mels, window_fn, wkwargs, center, norm, mel_scale,
                                             log_floor)
         self.params, self.fbank, self.window = params, fbank, window
         L = self.ctx._L
-        rates = np.array([f.info.sample_rate for f in corpus.index.files] or [0], dtype=np.uint32)
         h = C.c_void_p()
-        _check(L.clx_batch_create_mel_crops(self.ctx._h, corpus._h, rates.ctypes.data, len(corpus.index), self.batch,
-                                            self.num_frames, self.sample_rate or 0, C.byref(params),
+        _check(L.clx_batch_create_mel_crops(self.ctx._h, corpus._h, corpus._file_rates().ctypes.data, len(corpus.index),
+                                            self.batch, self.num_frames, self.sample_rate or 0, C.byref(params),
                                             window.ctypes.data, fbank.ctypes.data, C.byref(h)), self.ctx)
         self.channels, self.n_mels = corpus.channels, params.n_mels
         self.n_frames = (1 + self.num_frames // params.hop_length if center else
@@ -1497,8 +1496,9 @@ class MelCropBatch(CropBatch):
         self._attach(h, (self.batch, self.channels, self.n_mels, self.n_frames), "<f4")
 
 
-def _request_column(x, n: int | None, what: str):
-    """A request column as an int64 CUDA tensor (integers only; CPU values are copied through pinned memory)."""
+def _request_column(x, n: int | None, what: str, of_n: str = "{} files"):
+    """A request column as an int64 CUDA tensor (integers only; CPU values are copied through pinned memory) of n values
+    unless n is None; `of_n` names n in the error."""
     import torch
     if isinstance(x, torch.Tensor):
         if x.dtype.is_floating_point or x.dtype.is_complex or x.dtype == torch.bool:
@@ -1507,7 +1507,7 @@ def _request_column(x, n: int | None, what: str):
     else:
         t = torch.from_numpy(np.asarray(x, dtype=np.int64).reshape(-1))
     if n is not None and t.numel() != n:
-        raise ValueError(f"{what}: {t.numel()} values for {n} files")
+        raise ValueError(f"{what}: {t.numel()} values for {of_n.format(n)}")
     if not t.is_cuda:
         t = t.to(torch.int64).pin_memory().to("cuda", non_blocking=True)
     return t
@@ -1543,32 +1543,41 @@ class PackedBatch:
     r / R samples per row for the highest rate r: 6 x T for 96 kHz to 16 kHz)."""
 
     def __init__(self, corpus: Corpus, max_excerpts: int, max_samples: int, dtype=None, sample_rate: int | None = None):
-        import torch
-        dtype = _torch_dtype(dtype)
-        self.corpus, self.ctx = corpus, corpus.ctx
-        self.max_excerpts, self.max_samples, self.dtype = int(max_excerpts), int(max_samples), dtype
-        self.sample_rate = None if sample_rate is None else int(sample_rate)
-        if self.max_excerpts < 1 or self.max_samples < 1:
-            raise ValueError("max_excerpts and max_samples must be >= 1")
-        mode = _channels_mode(dtype)
+        mode = self._args(corpus, max_excerpts, max_samples, dtype, sample_rate)
         L = self.ctx._L
         h = C.c_void_p()
         if self.sample_rate is None:
             _check(L.clx_batch_create_packed(self.ctx._h, corpus._h, self.max_excerpts, self.max_samples, mode,
                                              C.byref(h)), self.ctx)
         else:
-            if dtype != torch.float32:
-                raise ValueError("a resampled packed batch is float32 only")
-            rates = np.array([f.info.sample_rate for f in corpus.index.files] or [0], dtype=np.uint32)
-            _check(L.clx_batch_create_resampled_packed(self.ctx._h, corpus._h, rates.ctypes.data, len(corpus.index),
-                                                       self.max_excerpts, self.max_samples, self.sample_rate,
-                                                       C.byref(h)), self.ctx)
-        self._batch = _Batch(self.ctx, h, keep=corpus)
+            _check(L.clx_batch_create_resampled_packed(self.ctx._h, corpus._h, corpus._file_rates().ctypes.data,
+                                                       len(corpus.index), self.max_excerpts, self.max_samples,
+                                                       self.sample_rate, C.byref(h)), self.ctx)
         self.channels = corpus.channels
+        self._attach(h, (self.channels,), "<f4" if mode == OUT_CHANNELS_F32 else "<i4")
+        self.out = self.out[:, :self.max_samples]
+
+    def _args(self, corpus: Corpus, max_excerpts: int, max_samples: int, dtype, sample_rate: int | None) -> int:
+        """Checks and keeps the arguments of every packed batch; returns the output mode."""
+        import torch
+        self.corpus, self.ctx = corpus, corpus.ctx
+        self.max_excerpts, self.max_samples, self.dtype = int(max_excerpts), int(max_samples), _torch_dtype(dtype)
+        self.sample_rate = None if sample_rate is None else int(sample_rate)
+        if self.max_excerpts < 1 or self.max_samples < 1:
+            raise ValueError("max_excerpts and max_samples must be >= 1")
+        if self.sample_rate is not None and self.dtype != torch.float32:
+            raise ValueError("a resampled packed batch is float32 only")
+        return _channels_mode(self.dtype)
+
+    def _attach(self, h, out_shape: tuple, typestr: str):
+        """Takes ownership of the created batch `h` and views its buffers: out (out_shape, then the batch's stride),
+        starts, lengths, status, requests, count, error."""
+        import torch
+        L = self.ctx._L
+        self._batch = _Batch(self.ctx, h, keep=self.corpus)
         self.stride = int(L.clx_batch_packed_stride(h))
         B, view = self.max_excerpts, self._batch.tensor
-        self.out = view(L.clx_batch_device_out(h), (self.channels, self.stride),
-                        "<f4" if mode == OUT_CHANNELS_F32 else "<i4")[:, :self.max_samples]
+        self.out = view(L.clx_batch_device_out(h), (*out_shape, self.stride), typestr)
         self._starts = view(L.clx_batch_packed_starts(h), (B,), "<i8")
         self._lengths = view(L.clx_batch_crop_lengths(h), (B,), "<i8")
         self._status = view(L.clx_batch_crop_status(h), (B,), "<i4")
@@ -1616,21 +1625,15 @@ class PackedBatch:
         return self.out, self._starts[:n], self._lengths[:n]
 
     def _raise(self):
-        err = int(self._error.item()) & ((1 << 64) - 1)  # the one sync
-        if err == (1 << 64) - 1:
+        failure = _first_failure(self._error)
+        if failure is None:
             return
-        kind, b, st = err >> 62, (err >> 32) & ((1 << 30) - 1), err & 0xffffffff
-        st = st - (1 << 32) if st >= 1 << 31 else st
+        kind, b, st = failure
         fi, o, ln = (int(v) for v in self._requests[b].tolist())
         if kind == 0:
             if not 0 <= fi < len(self.corpus.index):
                 raise ValueError(f"excerpt {b}: file index {fi} out of range")
-            f = self.corpus.index[fi]
-            N, at = f.length, ""
-            if self.sample_rate is not None and f.info.sample_rate != self.sample_rate:
-                g = math.gcd(f.info.sample_rate, self.sample_rate)
-                N = -(-f.length * (self.sample_rate // g) // (f.info.sample_rate // g))
-                at = f" at {self.sample_rate} Hz"
+            N, at = _length_at(self.corpus.index[fi], self.sample_rate)
             if not 0 <= o <= N:
                 raise ValueError(f"excerpt {b}: offset {o} outside file {fi} ({N} samples{at})")
             if ln == 0 or ln < -1:
@@ -1674,37 +1677,20 @@ class MelPackedBatch(PackedBatch):
                  n_fft: int = 400, win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
                  f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
                  center: bool = True, norm: str | None = None, mel_scale: str = "htk", log_floor: float | None = None):
-        import torch
-        self.corpus, self.ctx = corpus, corpus.ctx
-        self.max_excerpts, self.max_samples, self.dtype = int(max_excerpts), int(max_samples), torch.float32
-        self.sample_rate = None if sample_rate is None else int(sample_rate)
-        if self.max_excerpts < 1 or self.max_samples < 1:
-            raise ValueError("max_excerpts and max_samples must be >= 1")
+        self._args(corpus, max_excerpts, max_samples, None, sample_rate)
         params, window, fbank = _mel_tables(_mel_rate(corpus.index, self.sample_rate), n_fft, win_length, hop_length,
                                             f_min, f_max, n_mels, window_fn, wkwargs, center, norm, mel_scale,
                                             log_floor)
         self.params, self.fbank, self.window = params, fbank, window
         L = self.ctx._L
-        rates = np.array([f.info.sample_rate for f in corpus.index.files] or [0], dtype=np.uint32)
         h = C.c_void_p()
-        _check(L.clx_batch_create_mel_packed(self.ctx._h, corpus._h, rates.ctypes.data, len(corpus.index),
-                                             self.max_excerpts, self.max_samples, self.sample_rate or 0,
-                                             C.byref(params), window.ctypes.data, fbank.ctypes.data, C.byref(h)),
-               self.ctx)
-        self._batch = _Batch(self.ctx, h, keep=corpus)
+        _check(L.clx_batch_create_mel_packed(self.ctx._h, corpus._h, corpus._file_rates().ctypes.data,
+                                             len(corpus.index), self.max_excerpts, self.max_samples,
+                                             self.sample_rate or 0, C.byref(params), window.ctypes.data,
+                                             fbank.ctypes.data, C.byref(h)), self.ctx)
         self.channels, self.n_mels = corpus.channels, params.n_mels
-        self.stride = int(L.clx_batch_packed_stride(h))  # T_f
-        B, view = self.max_excerpts, self._batch.tensor
-        self.out = view(L.clx_batch_device_out(h), (self.channels, self.n_mels, self.stride), "<f4")
-        self._starts = view(L.clx_batch_packed_starts(h), (B,), "<i8")
-        self._frames = view(L.clx_batch_mel_frames(h), (B,), "<i8")
-        self._lengths = view(L.clx_batch_crop_lengths(h), (B,), "<i8")
-        self._status = view(L.clx_batch_crop_status(h), (B,), "<i4")
-        self._requests = view(L.clx_batch_packed_requests(h), (B, 3), "<i8")
-        self._count = view(L.clx_batch_packed_count(h), (1,), "<i4")
-        self._error = view(L.clx_batch_crop_error(h), (1,), "<i8")
-        self._stream = torch.cuda.ExternalStream(L.clx_ctx_stream(self.ctx._h, 0))
-        self._n = 0
+        self._attach(h, (self.channels, self.n_mels), "<f4")  # stride: T_f
+        self._frames = self._batch.tensor(L.clx_batch_mel_frames(h), (self.max_excerpts,), "<i8")
 
     def __call__(self, files, offsets=None, lengths=None, check: bool = True):
         """Computes the features of excerpt b = samples [offsets[b], offsets[b] + lengths[b]) of file files[b], cut at

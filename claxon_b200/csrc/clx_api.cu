@@ -198,6 +198,9 @@ struct clx_ctx {
 };
 
 struct clx_batch {
+    // What the batch decodes: frames it was given, or one of the corpus kinds (clx_batch_create_crops ... _mel_packed).
+    enum class Kind { Frames, Crops, Packed, ResampledCrops, ResampledPacked, MelCrops, MelPacked };
+    Kind kind = Kind::Frames;
     DecodeStorage buf;
     size_t out_elems = 0;
     uint32_t n_frames = 0;
@@ -225,29 +228,19 @@ struct clx_batch {
     // windows for clx_batch_create_channels), both in the device order.
     uint32_t mode = CLX_OUT_PLANAR_I32;
     uint64_t stride = 0;
-    // Crop batches (clx_batch_create_crops): buf.bytes is the corpus's, not the batch's; the planner writes buf.descs,
-    // buf.cols and buf.wins in every decode (clx_crops.cu).  Over a host corpus, buf.bytes is the batch's own staging
-    // buffer: n_crops spans of span_stride bytes, then the filler frame.
-    // Packed batches (clx_batch_create_packed) are crop batches with `packed` set: crop holds their per-excerpt plan,
-    // status, lengths, error word and slot scan, and over a host corpus span_stride is the staging bound, after which
-    // the filler frame is staged.
+    // Corpus batches.  Crops and Packed decode frames of `corpus`: buf.bytes is the corpus's, or over a host corpus the
+    // batch's own staging buffer (span_stride apart per crop, or the staging bound of a packed batch), the filler frame
+    // after it; the planner writes buf.descs, buf.cols and buf.wins in every decode (clx_crops.cu).  The other kinds
+    // wrap `inner`, whose launch sequence runs inside theirs, and write their output to buf.conv.  The buffers below
+    // are the kinds' device state; a wrapper's may point into its inner batch's.  `owned` lists every device allocation
+    // of the batch outside `buf`, which is all clx_batch_destroy frees besides `buf` and `inner`.
     clx_corpus* corpus = nullptr;
+    std::vector<void*> owned;
     clx::CropBuffers crop{};
     uint64_t span_stride = 0;
-    bool is_packed = false;
     clx::PackedBuffers packed{};
-    // Resampled crop batches (clx_batch_create_resampled_crops): crop batches whose graph runs `inner`, a packed batch,
-    // between the map and filter kernels.  crop.requests and crop.lengths are their own, crop.status and crop.error
-    // the inner batch's; buf.conv is the output; rs the rest.  Resampled packed batches
-    // (clx_batch_create_resampled_packed) are those with `packed` set too: packed holds their own requests, count and
-    // target column starts (its other buffers stay null), and crop.requests is null.
     clx_batch* inner = nullptr;
     clx::ResampleBuffers rs{};
-    // Mel crop batches (clx_batch_create_mel_crops): `inner` is a crop or resampled crop batch, run before mel_kernel.
-    // crop.requests, status, lengths and error are the inner batch's; buf.conv is the features; mel the rest.  Mel
-    // packed batches (clx_batch_create_mel_packed) are those with `packed` set too: `inner` is a packed or resampled
-    // packed batch, packed.requests and count are its own, packed.starts the frame starts, and mel_packed the rest.
-    bool is_mel = false;
     clx::MelBuffers mel{};
     size_t mel_smem = 0;
     clx::MelPacked mel_packed{};
@@ -314,7 +307,7 @@ void precompute_crc(clx_ctx* ctx, const uint8_t* bytes, const clx_frame_desc* de
     });
 }
 
-void build_graph(clx_ctx* ctx, clx_batch* b);
+int finish(clx_ctx* ctx, clx_batch* b, cudaError_t e, const char* what, clx_batch** out);
 
 // Where a create or decode call writes its `out_elems` samples.  Planar and interleaved modes: each frame from its
 // out_offset on.  Channels modes: `n_rows` rows of `stride` elements; frame i stores its window windows[i] (null: every
@@ -676,53 +669,44 @@ int create_batch(clx_ctx* ctx, const uint8_t* bytes, size_t nbytes, const clx_fr
     if (e == cudaSuccess) e = cudaMemcpy(b->buf.bytes, bytes, nbytes, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
     if (e == cudaSuccess)
         e = cudaMemcpy(b->buf.descs, dev.empty() ? descs : dev.data(), n_frames * sizeof(clx_frame_desc), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
-    if (e != cudaSuccess) {
-        clx_batch_destroy(ctx, b);
-        return cuda_fail(ctx, e, "clx_batch_create");
-    }
-    if (!(ctx->flags & CLX_OPT_NO_VERIFY_CRC)) {
+    if (e == cudaSuccess && !(ctx->flags & CLX_OPT_NO_VERIFY_CRC)) {
         if (on_device) b->device_crc = true;  // no host copy to checksum: clx_crc.cu, as part of every decode
         else precompute_crc(ctx, bytes, descs, n_frames, b->crc_ok);
     }
     b->h_offset.resize(n_frames);
     b->h_len.resize(n_frames);
     for (size_t i = 0; i < n_frames; i++) { b->h_offset[i] = descs[i].byte_offset; b->h_len[i] = descs[i].byte_len; }
-    build_graph(ctx, b);
-    *out = b;
-    return CLX_OK;
+    return finish(ctx, b, e, "clx_batch_create", out);
 }
 
 cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
+    using Kind = clx_batch::Kind;
     const clx::DecodeBuffers db = b->buf.view(b->n_frames, b->mode, b->stride);
-    if (b->is_mel) {
-        cudaError_t e = launch_batch(b->inner, st, launches);
-        if (e == cudaSuccess)
-            e = b->is_packed ? clx::launch_mel_packed(b->mel, b->mel_packed, b->mel_smem, st, launches)
-                             : clx::launch_mel(b->mel, b->mel_smem, st, launches);
-        return e;
-    }
-    if (b->inner && b->is_packed) {
-        const clx::CropCorpus cc = b->corpus->view(0);
-        cudaError_t e = clx::launch_resample_packed_map(cc, b->rs, b->packed, st, launches);
-        if (e == cudaSuccess) e = launch_batch(b->inner, st, launches);
-        if (e == cudaSuccess) e = clx::launch_resample_packed(b->rs, b->packed, st, launches);
-        return e;
-    }
-    if (b->inner) {
-        const clx::CropCorpus cc = b->corpus->view(0);
-        cudaError_t e = clx::launch_resample_map(cc, b->rs, st, launches);
-        if (e == cudaSuccess) e = launch_batch(b->inner, st, launches);
-        if (e == cudaSuccess) e = clx::launch_resample(b->rs, st, launches);
-        return e;
-    }
-    if (b->corpus && b->is_packed)
+    cudaError_t e = cudaSuccess;
+    switch (b->kind) {
+    case Kind::Frames:
+        return clx::launch_decode(db, b->plan, b->device_crc, st, launches);
+    case Kind::Crops:
+        return clx::launch_crops(b->corpus->view(b->span_stride), b->crop, db, b->plan, b->device_crc, st, launches);
+    case Kind::Packed:
         return clx::launch_packed(b->corpus->view(b->span_stride), b->crop, b->packed, db, b->plan, b->device_crc, st,
                                   launches);
-    if (b->corpus)
-        return clx::launch_crops(b->corpus->view(b->span_stride), b->crop, db, b->plan, b->device_crc, st, launches);
-    return clx::launch_decode(db, b->plan, b->device_crc, st, launches);
+    case Kind::ResampledCrops:
+        e = clx::launch_resample_map(b->corpus->view(0), b->rs, st, launches);
+        if (e == cudaSuccess) e = launch_batch(b->inner, st, launches);
+        return e == cudaSuccess ? clx::launch_resample(b->rs, st, launches) : e;
+    case Kind::ResampledPacked:
+        e = clx::launch_resample_packed_map(b->corpus->view(0), b->rs, b->packed, st, launches);
+        if (e == cudaSuccess) e = launch_batch(b->inner, st, launches);
+        return e == cudaSuccess ? clx::launch_resample_packed(b->rs, b->packed, st, launches) : e;
+    case Kind::MelCrops:
+        e = launch_batch(b->inner, st, launches);
+        return e == cudaSuccess ? clx::launch_mel(b->mel, b->mel_smem, st, launches) : e;
+    case Kind::MelPacked:
+        e = launch_batch(b->inner, st, launches);
+        return e == cudaSuccess ? clx::launch_mel_packed(b->mel, b->mel_packed, b->mel_smem, st, launches) : e;
+    }
+    return cudaErrorInvalidValue;
 }
 
 // Captures the batch's launch sequence once; called from clx_batch_create so that no decode ever pays for
@@ -747,6 +731,21 @@ void build_graph(clx_ctx* ctx, clx_batch* b) {
         b->graph = nullptr;
         cudaGetLastError();
     } else b->graph_launches = n;
+}
+
+// The end of every public create, after the batch's buffers were made with the first CUDA error `e`: its timing events
+// and its graph, or on an error none of it (the batch is destroyed).  An inner batch is never finished: the graph of
+// the batch around it launches its kernels.
+int finish(clx_ctx* ctx, clx_batch* b, cudaError_t e, const char* what, clx_batch** out) {
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
+    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
+    if (e != cudaSuccess) {
+        clx_batch_destroy(ctx, b);
+        return cuda_fail(ctx, e, what);
+    }
+    build_graph(ctx, b);
+    *out = b;
+    return CLX_OK;
 }
 
 // Enqueues one decode of a device-resident batch on `st`, through the batch's graph when there is one.
@@ -845,28 +844,9 @@ void clx_batch_destroy(clx_ctx* ctx, clx_batch* b) {
     (void)ctx;
     if (!b) return;
     b->buf.release();
-    if (b->is_mel) {
-        b->crop.requests = nullptr;  // the inner batch's, as status and error below
-        b->crop.lengths = nullptr;
-        b->packed.requests = nullptr;
-        b->packed.count = nullptr;
-        cudaFree((void*)b->mel.tw); cudaFree((void*)b->mel.window); cudaFree((void*)b->mel.bands);
-        cudaFree((void*)b->mel.weights); cudaFree(b->mel_packed.frames);
-    }
-    if (b->inner) {
-        b->crop.status = nullptr;  // the inner batch's
-        b->crop.error = nullptr;
-        cudaFree(b->rs.plan); cudaFree((void*)b->rs.file_rate); cudaFree((void*)b->rs.rates); cudaFree((void*)b->rs.coefs);
-        cudaFree((void*)b->rs.k0);
-        clx_batch_destroy(ctx, b->inner);
-    }
-    if (b->corpus) {
-        b->corpus->live--;
-        cudaFree((void*)b->crop.requests); cudaFree(b->crop.status); cudaFree(b->crop.lengths); cudaFree(b->crop.error);
-        cudaFree(b->crop.plan); cudaFree(b->crop.scan);
-        cudaFree((void*)b->packed.requests); cudaFree((void*)b->packed.count); cudaFree(b->packed.starts);
-        cudaFree(b->packed.stage); cudaFree(b->packed.chunks); cudaFree(b->packed.end);
-    }
+    for (void* p : b->owned) cudaFree(p);
+    clx_batch_destroy(ctx, b->inner);
+    if (b->corpus) b->corpus->live--;
     if (b->graph) cudaGraphExecDestroy(b->graph);
     if (b->ev_idle) cudaEventDestroy(b->ev_idle);
     if (b->ev_start) cudaEventDestroy(b->ev_start);
@@ -1145,64 +1125,101 @@ size_t clx_corpus_device_bytes(const clx_corpus* corpus) { return corpus ? corpu
 }  // extern "C"
 
 namespace {
-template <typename T>
-cudaError_t device_zeros(T*& p, size_t n) {
-    cudaError_t e = cudaMalloc((void**)&p, n * sizeof(T));
-    return e == cudaSuccess ? cudaMemset((void*)p, 0, n * sizeof(T)) : e;
+using Kind = clx_batch::Kind;
+
+// A batch of a corpus kind, counted by the corpus until clx_batch_destroy; a wrapper's `inner` is destroyed with it.
+clx_batch* new_batch(Kind kind, clx_corpus* corpus, clx_batch* inner = nullptr) {
+    clx_batch* b = new clx_batch();
+    b->kind = kind;
+    b->corpus = corpus;
+    b->inner = inner;
+    corpus->live++;
+    return b;
 }
+
+// A device array of n elements that b owns: uninitialised (device_alloc) or zeroed (device_zeros).
 template <typename T>
-cudaError_t device_zeros(const T*& p, size_t n) {
-    T* q = nullptr;
-    const cudaError_t e = device_zeros(q, n);
-    p = q;
+cudaError_t device_alloc(clx_batch* b, T*& p, size_t n) {
+    void* q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, n * sizeof(T));
+    if (e == cudaSuccess) b->owned.push_back(q);
+    p = static_cast<T*>(q);
     return e;
 }
-// A device copy of a host table (one element at least, so that an empty table is a valid pointer too).
 template <typename T>
-cudaError_t upload(const T*& p, const std::vector<T>& v) {
+cudaError_t device_zeros(clx_batch* b, T*& p, size_t n) {
+    const cudaError_t e = device_alloc(b, p, n);
+    return e == cudaSuccess ? cudaMemset((void*)p, 0, n * sizeof(T)) : e;
+}
+// A device copy of a host table that b owns (one element at least, so that an empty table is a valid pointer too).
+template <typename T>
+cudaError_t upload(clx_batch* b, const T*& p, const std::vector<T>& v) {
     T* q = nullptr;
-    cudaError_t e = cudaMalloc((void**)&q, std::max<size_t>(v.size(), 1) * sizeof(T));
+    cudaError_t e = device_alloc(b, q, std::max<size_t>(v.size(), 1));
     p = q;
     if (e == cudaSuccess && !v.empty()) e = cudaMemcpy(q, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
     return e;
 }
+// A wrapper's float32 output in buf.conv, zeroed, with the slack of DecodeStorage::fit (buf.release() frees it).
+cudaError_t alloc_output(clx_batch* b) {
+    const size_t bytes = (b->out_elems + 8) * sizeof(float);
+    const cudaError_t e = cudaMalloc((void**)&b->buf.conv, bytes);
+    return e == cudaSuccess ? cudaMemset(b->buf.conv, 0, bytes) : e;
+}
 
-// The per-excerpt buffers every crop or packed batch's planner writes (all but the requests), and its timing events.
-cudaError_t alloc_planner(clx_batch* b, size_t n) {
+// Crop and packed batches: the corpus and mode they accept; their decode plan (every frame of the corpus, the filler
+// frame included) and its planar elements per slot.
+bool planned_ok(const clx_ctx* ctx, const clx_corpus* corpus, uint32_t mode) {
+    return ctx && corpus && is_channels(mode) && !(mode == CLX_OUT_CHANNELS_F32 && corpus->max_bps > 24);
+}
+clx::Plan corpus_plan(const clx_ctx* ctx, const clx_corpus* corpus, size_t* slot_elems) {
+    const clx::Plan plan = make_plan(ctx, corpus->descs.data(), corpus->descs.size());
+    *slot_elems = ((size_t)plan.max_frame_elems + 3) & ~(size_t)3;
+    return plan;
+}
+// The buffers crop and packed batches share, once the kind has set b->crop's sizes and b->span_stride: the frame bytes
+// (the corpus's, or over a host corpus `staged` bytes of staging and then the filler frame), the slots' planar scratch,
+// an output of conv_elems elements (trash included), and the planner's per-excerpt buffers.
+cudaError_t alloc_planned(clx_ctx* ctx, clx_batch* b, const clx::Plan& plan, uint32_t mode, size_t staged,
+                          size_t conv_elems) {
+    const clx_corpus* c = b->corpus;
     clx::CropBuffers& cb = b->crop;
-    cudaError_t e = device_zeros(cb.status, n);
-    if (e == cudaSuccess) e = device_zeros(cb.lengths, n);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.error, sizeof(unsigned long long));
+    const size_t n = cb.n_crops, filler_len = clx::filler_frame(nullptr, 0);
+    b->n_frames = cb.n_slots;
+    b->plan = plan;
+    b->mode = mode;
+    b->device_crc = !(ctx->flags & CLX_OPT_NO_VERIFY_CRC);
+    if (!c->h_bytes) b->buf.borrow(c->d_bytes, c->buf_bytes);
+    cudaError_t e = b->buf.fit({staged + filler_len, cb.n_slots, cb.n_slots * cb.slot_elems, mode, conv_elems, true, plan},
+                               false);
+    if (e == cudaSuccess && c->h_bytes)
+        e = cudaMemcpy(b->buf.bytes + staged, c->h_bytes + c->nbytes, filler_len, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = device_zeros(b, cb.status, n);
+    if (e == cudaSuccess) e = device_zeros(b, cb.lengths, n);
+    if (e == cudaSuccess) e = device_alloc(b, cb.error, 1);
     if (e == cudaSuccess) e = cudaMemset(cb.error, 0xff, sizeof(unsigned long long));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.plan, n * sizeof(clx::CropPlan));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&cb.scan, (n + 1) * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
+    if (e == cudaSuccess) e = device_alloc(b, cb.plan, n);
+    if (e == cudaSuccess) e = device_alloc(b, cb.scan, n + 1);
     return e;
 }
-}  // namespace
 
-extern "C" {
-
-int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, size_t num_frames, uint32_t mode,
-                           clx_batch** out) {
-    if (!out) return CLX_ERR_INVALID_ARGUMENT;
-    *out = nullptr;
-    if (!ctx || !corpus || n_crops == 0 || num_frames == 0 || n_crops >= (1u << 30) ||
-        !is_channels(mode) || (mode == CLX_OUT_CHANNELS_F32 && corpus->max_bps > 24))
+// The first half of each corpus batch's create (finish() is the second): a refusal, or CLX_OK with *out the batch and
+// *e the first CUDA error of making its buffers.  A wrapper makes its inner batch the same way.
+int make_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, size_t num_frames, uint32_t mode, clx_batch** out,
+               cudaError_t* e) {
+    if (!planned_ok(ctx, corpus, mode) || n_crops == 0 || num_frames == 0 || n_crops >= (1u << 30))
         return CLX_ERR_INVALID_ARGUMENT;
     const size_t S = clx_crop_frames_bound(corpus->descs.data(), corpus->n_frames, corpus->file_frames.data(),
                                            corpus->n_files, num_frames);
     const size_t C = corpus->channels, rows = n_crops * C;  // (< 2^33: no overflow)
-    const clx::Plan plan = make_plan(ctx, corpus->descs.data(), corpus->descs.size());
-    const size_t slot_elems = ((size_t)plan.max_frame_elems + 3) & ~(size_t)3;
+    size_t slot_elems;
+    const clx::Plan plan = corpus_plan(ctx, corpus, &slot_elems);
     if (S == 0 || S > UINT32_MAX / n_crops || num_frames > (SIZE_MAX / 4 - 8) / (rows + C)) return CLX_ERR_INVALID_ARGUMENT;
     const size_t slots = n_crops * S;
     if (slots > (SIZE_MAX / 4 - 8) / slot_elems) return CLX_ERR_INVALID_ARGUMENT;
     // Over a host corpus, the batch's own frame bytes: crop b's span at b * span_stride + (its start & 15), then the
     // filler frame after the last span.
     size_t span_stride = 0;
-    const size_t filler_len = clx::filler_frame(nullptr, 0);
     if (corpus->h_bytes) {
         const size_t span = clx_crop_bytes_bound(corpus->descs.data(), corpus->n_frames, corpus->file_frames.data(),
                                                  corpus->n_files, num_frames);
@@ -1210,17 +1227,10 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
         if (span_stride > (SIZE_MAX / 2) / n_crops) return CLX_ERR_INVALID_ARGUMENT;
     }
     CU(ctx, cudaSetDevice(ctx->device));
-    clx_batch* b = new clx_batch();
-    b->corpus = corpus;
-    corpus->live++;
-    if (!corpus->h_bytes) b->buf.borrow(corpus->d_bytes, corpus->buf_bytes);
+    clx_batch* b = *out = new_batch(Kind::Crops, corpus);
     b->span_stride = span_stride;
-    b->n_frames = (uint32_t)slots;
     b->out_elems = rows * num_frames;
-    b->plan = plan;
-    b->mode = mode;
     b->stride = num_frames;
-    b->device_crc = !(ctx->flags & CLX_OPT_NO_VERIFY_CRC);
     clx::CropBuffers& cb = b->crop;
     cb.n_crops = (uint32_t)n_crops;
     cb.C = (uint32_t)C;
@@ -1229,33 +1239,15 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
     cb.L = num_frames;
     cb.slot_elems = slot_elems;
     // the output plus C trash rows for the unused slots
-    cudaError_t e = b->buf.fit({n_crops * span_stride + filler_len, slots, slots * slot_elems, mode, (rows + C) * num_frames,
-                                true, plan}, false);
-    if (e == cudaSuccess && corpus->h_bytes)
-        e = cudaMemcpy(b->buf.bytes + n_crops * span_stride, corpus->h_bytes + corpus->nbytes, filler_len,
-                       cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = device_zeros(cb.requests, n_crops);
-    if (e == cudaSuccess) e = alloc_planner(b, n_crops);
-    if (e != cudaSuccess) {
-        clx_batch_destroy(ctx, b);
-        return cuda_fail(ctx, e, "clx_batch_create_crops");
-    }
-    build_graph(ctx, b);
-    *out = b;
+    *e = alloc_planned(ctx, b, plan, mode, n_crops * span_stride, (rows + C) * num_frames);
+    if (*e == cudaSuccess) *e = device_zeros(b, cb.requests, n_crops);
     return CLX_OK;
 }
 
-void* clx_batch_crop_requests(clx_batch* b) { return b && b->corpus ? (void*)b->crop.requests : nullptr; }
-void* clx_batch_crop_status(clx_batch* b) { return b && b->corpus ? (void*)b->crop.status : nullptr; }
-void* clx_batch_crop_lengths(clx_batch* b) { return b && b->corpus ? (void*)b->crop.lengths : nullptr; }
-void* clx_batch_crop_error(clx_batch* b) { return b && b->corpus ? (void*)b->crop.error : nullptr; }
-
-int clx_batch_create_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpts, size_t max_samples, uint32_t mode,
-                            clx_batch** out) {
-    if (!out) return CLX_ERR_INVALID_ARGUMENT;
-    *out = nullptr;
-    if (!ctx || !corpus || max_excerpts == 0 || max_samples == 0 || max_excerpts >= (1u << 30) ||
-        max_samples > SIZE_MAX / 16 || !is_channels(mode) || (mode == CLX_OUT_CHANNELS_F32 && corpus->max_bps > 24))
+int make_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpts, size_t max_samples, uint32_t mode,
+                clx_batch** out, cudaError_t* e) {
+    if (!planned_ok(ctx, corpus, mode) || max_excerpts == 0 || max_samples == 0 || max_excerpts >= (1u << 30) ||
+        max_samples > SIZE_MAX / 16)
         return CLX_ERR_INVALID_ARGUMENT;
     const clx_frame_desc* descs = corpus->descs.data();
     const uint32_t* ff = corpus->file_frames.data();
@@ -1264,32 +1256,23 @@ int clx_batch_create_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpt
     for (const clx_frame_desc& d : corpus->descs) largest = std::max<uint32_t>(largest, d.block_size);
     const size_t T4 = (max_samples + 3) & ~(size_t)3, W = (std::min<size_t>(max_samples, largest) + 3) & ~(size_t)3;
     const size_t C = corpus->channels, stride = T4 + W;
-    const clx::Plan plan = make_plan(ctx, descs, corpus->descs.size());
-    const size_t slot_elems = ((size_t)plan.max_frame_elems + 3) & ~(size_t)3;
+    size_t slot_elems;
+    const clx::Plan plan = corpus_plan(ctx, corpus, &slot_elems);
     if (S == 0 || S >= UINT32_MAX || stride > (SIZE_MAX / 4 - 8) / C || S > (SIZE_MAX / 4 - 8) / slot_elems)
         return CLX_ERR_INVALID_ARGUMENT;
     // Over a host corpus, the batch's own frame bytes: the excerpts' spans packed from 0 (at most the bytes bound), then
     // the filler frame.
     size_t span_stride = 0, chunks = 0;
-    const size_t filler_len = clx::filler_frame(nullptr, 0);
     if (corpus->h_bytes) {
         span_stride = clx_packed_bytes_bound(descs, corpus->n_frames, ff, corpus->n_files, max_excerpts, max_samples);
         if (span_stride > SIZE_MAX / 2) return CLX_ERR_INVALID_ARGUMENT;
         chunks = span_stride / (16 * 1024) + max_excerpts;  // ceil(span / GATHER_CHUNK) per excerpt, every span together
     }
     CU(ctx, cudaSetDevice(ctx->device));
-    clx_batch* b = new clx_batch();
-    b->corpus = corpus;
-    corpus->live++;
-    b->is_packed = true;
-    if (!corpus->h_bytes) b->buf.borrow(corpus->d_bytes, corpus->buf_bytes);
+    clx_batch* b = *out = new_batch(Kind::Packed, corpus);
     b->span_stride = span_stride;
-    b->n_frames = (uint32_t)S;
     b->out_elems = C * stride;
-    b->plan = plan;
-    b->mode = mode;
     b->stride = stride;
-    b->device_crc = !(ctx->flags & CLX_OPT_NO_VERIFY_CRC);
     clx::CropBuffers& cb = b->crop;
     cb.n_crops = (uint32_t)max_excerpts;
     cb.C = (uint32_t)C;
@@ -1302,34 +1285,53 @@ int clx_batch_create_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpt
     pb.W = W;
     pb.max_chunks = (uint32_t)std::min<size_t>(std::max<size_t>(chunks, 1), 1u << 20);
     // the output with its trash columns, zeroed here: afterwards every call zeroes what it must
-    cudaError_t e = b->buf.fit({span_stride + filler_len, S, S * slot_elems, mode, C * stride, true, plan}, false);
-    if (e == cudaSuccess && corpus->h_bytes)
-        e = cudaMemcpy(b->buf.bytes + span_stride, corpus->h_bytes + corpus->nbytes, filler_len, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = device_zeros(pb.requests, max_excerpts);
-    if (e == cudaSuccess) e = device_zeros(pb.count, 1);
-    if (e == cudaSuccess) e = device_zeros(pb.starts, max_excerpts);
-    if (e == cudaSuccess) e = device_zeros(pb.stage, max_excerpts);
-    if (e == cudaSuccess) e = device_zeros(pb.chunks, max_excerpts + 1);
-    if (e == cudaSuccess) e = device_zeros(pb.end, 2);
-    if (e == cudaSuccess) e = alloc_planner(b, max_excerpts);
-    if (e != cudaSuccess) {
-        clx_batch_destroy(ctx, b);
-        return cuda_fail(ctx, e, "clx_batch_create_packed");
-    }
-    build_graph(ctx, b);
-    *out = b;
+    *e = alloc_planned(ctx, b, plan, mode, span_stride, C * stride);
+    if (*e == cudaSuccess) *e = device_zeros(b, pb.requests, max_excerpts);
+    if (*e == cudaSuccess) *e = device_zeros(b, pb.count, 1);
+    if (*e == cudaSuccess) *e = device_zeros(b, pb.starts, max_excerpts);
+    if (*e == cudaSuccess) *e = device_zeros(b, pb.stage, max_excerpts);
+    if (*e == cudaSuccess) *e = device_zeros(b, pb.chunks, max_excerpts + 1);
+    if (*e == cudaSuccess) *e = device_zeros(b, pb.end, 2);
     return CLX_OK;
 }
 
-void* clx_batch_packed_requests(clx_batch* b) { return b && b->is_packed ? (void*)b->packed.requests : nullptr; }
-void* clx_batch_packed_count(clx_batch* b) { return b && b->is_packed ? (void*)b->packed.count : nullptr; }
-void* clx_batch_packed_starts(clx_batch* b) { return b && b->is_packed ? (void*)b->packed.starts : nullptr; }
-size_t clx_batch_packed_stride(clx_batch* b) { return b && b->is_packed ? b->stride : 0; }
+// Resampled crop and packed batches, once the kind has set b->out_elems: the filter of n excerpts of C rows into rows
+// of L outputs, with the tables `t`, reading the inner packed batch's source spans.  Status and error word are the
+// inner batch's, the lengths at the target rate the batch's own.
+cudaError_t fill_resample(clx_batch* b, const clx::ResampleTables& t, size_t n, size_t C, uint64_t L) {
+    const clx_batch* inner = b->inner;
+    b->mode = CLX_OUT_CHANNELS_F32;
+    b->stride = L;
+    clx::CropBuffers& cb = b->crop;
+    cb.n_crops = (uint32_t)n;
+    cb.C = (uint32_t)C;
+    cb.L = L;
+    cb.status = inner->crop.status;
+    cb.error = inner->crop.error;
+    clx::ResampleBuffers& rs = b->rs;
+    rs.n_crops = (uint32_t)n;
+    rs.C = (uint32_t)C;
+    rs.L = L;
+    rs.tile = t.tile;
+    rs.excerpts = const_cast<clx_packed_request*>(inner->packed.requests);
+    rs.count = const_cast<uint32_t*>(inner->packed.count);
+    rs.starts = inner->packed.starts;
+    rs.src = static_cast<const float*>((const void*)inner->buf.conv);
+    rs.src_stride = inner->stride;
+    cudaError_t e = device_zeros(b, cb.lengths, n);
+    if (e == cudaSuccess) e = alloc_output(b);
+    if (e == cudaSuccess) e = device_alloc(b, rs.plan, n);
+    if (e == cudaSuccess) e = upload(b, rs.file_rate, t.file_rate);
+    if (e == cudaSuccess) e = upload(b, rs.rates, t.rates);
+    if (e == cudaSuccess) e = upload(b, rs.coefs, t.coefs);
+    if (e == cudaSuccess) e = upload(b, rs.k0, t.k0);
+    rs.lengths = cb.lengths;
+    rs.out = reinterpret_cast<float*>(b->buf.conv);
+    return e;
+}
 
-int clx_batch_create_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
-                                     size_t n_crops, size_t num_frames, uint32_t target_rate, clx_batch** out) {
-    if (!out) return CLX_ERR_INVALID_ARGUMENT;
-    *out = nullptr;
+int make_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files, size_t n_crops,
+                         size_t num_frames, uint32_t target_rate, clx_batch** out, cudaError_t* e) {
     if (!ctx || !corpus || !file_rates || n_files != corpus->n_files || n_crops == 0 || num_frames == 0 ||
         n_crops >= (1u << 30))
         return CLX_ERR_INVALID_ARGUMENT;
@@ -1341,59 +1343,20 @@ int clx_batch_create_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uin
         (num_frames + t.tile - 1) / t.tile >= (1u << 31))
         return CLX_ERR_INVALID_ARGUMENT;
     clx_batch* inner = nullptr;
-    const int rc = clx_batch_create_packed(ctx, corpus, n_crops, n_crops * ((t.bound + 3) & ~(size_t)3),
-                                           CLX_OUT_CHANNELS_F32, &inner);
+    const int rc = make_packed(ctx, corpus, n_crops, n_crops * ((t.bound + 3) & ~(size_t)3), CLX_OUT_CHANNELS_F32,
+                               &inner, e);
     if (rc != CLX_OK) return rc;
-    clx_batch* b = new clx_batch();
-    b->corpus = corpus;
-    corpus->live++;
-    b->inner = inner;
+    clx_batch* b = *out = new_batch(Kind::ResampledCrops, corpus, inner);
     b->out_elems = rows * num_frames;
-    b->mode = CLX_OUT_CHANNELS_F32;
-    b->stride = num_frames;
-    clx::CropBuffers& cb = b->crop;
-    cb.n_crops = (uint32_t)n_crops;
-    cb.C = (uint32_t)C;
-    cb.L = num_frames;
-    cb.status = inner->crop.status;
-    cb.error = inner->crop.error;
-    clx::ResampleBuffers& rs = b->rs;
-    rs.n_crops = (uint32_t)n_crops;
-    rs.C = (uint32_t)C;
-    rs.L = num_frames;
-    rs.tile = t.tile;
-    rs.excerpts = const_cast<clx_packed_request*>(inner->packed.requests);
-    rs.count = const_cast<uint32_t*>(inner->packed.count);
-    rs.starts = inner->packed.starts;
-    rs.src = static_cast<const float*>((const void*)inner->buf.conv);
-    rs.src_stride = inner->stride;
-    cudaError_t e = cudaSetDevice(ctx->device);
-    if (e == cudaSuccess) e = device_zeros(cb.requests, n_crops);
-    if (e == cudaSuccess) e = device_zeros(cb.lengths, n_crops);
-    if (e == cudaSuccess) e = device_zeros(b->buf.conv, (b->out_elems + 8) * sizeof(float));  // (the slack of fit())
-    if (e == cudaSuccess) e = cudaMalloc((void**)&rs.plan, n_crops * sizeof(clx::ResamplePlan));
-    if (e == cudaSuccess) e = upload(rs.file_rate, t.file_rate);
-    if (e == cudaSuccess) e = upload(rs.rates, t.rates);
-    if (e == cudaSuccess) e = upload(rs.coefs, t.coefs);
-    if (e == cudaSuccess) e = upload(rs.k0, t.k0);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
-    if (e != cudaSuccess) {
-        clx_batch_destroy(ctx, b);
-        return cuda_fail(ctx, e, "clx_batch_create_resampled_crops");
-    }
-    rs.requests = cb.requests;
-    rs.lengths = cb.lengths;
-    rs.out = reinterpret_cast<float*>(b->buf.conv);
-    build_graph(ctx, b);
-    *out = b;
+    if (*e == cudaSuccess) *e = fill_resample(b, t, n_crops, C, num_frames);
+    if (*e == cudaSuccess) *e = device_zeros(b, b->crop.requests, n_crops);
+    b->rs.requests = b->crop.requests;
     return CLX_OK;
 }
 
-int clx_batch_create_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
-                                      size_t max_excerpts, size_t max_samples, uint32_t target_rate, clx_batch** out) {
-    if (!out) return CLX_ERR_INVALID_ARGUMENT;
-    *out = nullptr;
+int make_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                          size_t max_excerpts, size_t max_samples, uint32_t target_rate, clx_batch** out,
+                          cudaError_t* e) {
     if (!ctx || !corpus || !file_rates || n_files != corpus->n_files || max_excerpts == 0 || max_samples == 0 ||
         max_excerpts >= (1u << 30) || max_samples > SIZE_MAX / 16)
         return CLX_ERR_INVALID_ARGUMENT;
@@ -1405,63 +1368,55 @@ int clx_batch_create_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const ui
     if (src_cols == SIZE_MAX || stride > (SIZE_MAX / 4 - 8) / C || (stride + t.tile - 1) / t.tile >= (1u << 31))
         return CLX_ERR_INVALID_ARGUMENT;
     clx_batch* inner = nullptr;
-    const int rc = clx_batch_create_packed(ctx, corpus, max_excerpts, src_cols, CLX_OUT_CHANNELS_F32, &inner);
+    const int rc = make_packed(ctx, corpus, max_excerpts, src_cols, CLX_OUT_CHANNELS_F32, &inner, e);
     if (rc != CLX_OK) return rc;
-    clx_batch* b = new clx_batch();
-    b->corpus = corpus;
-    corpus->live++;
-    b->inner = inner;
-    b->is_packed = true;
+    clx_batch* b = *out = new_batch(Kind::ResampledPacked, corpus, inner);
     b->out_elems = C * stride;
-    b->mode = CLX_OUT_CHANNELS_F32;
-    b->stride = stride;
-    clx::CropBuffers& cb = b->crop;
-    cb.n_crops = (uint32_t)max_excerpts;
-    cb.C = (uint32_t)C;
-    cb.L = stride;
-    cb.status = inner->crop.status;
-    cb.error = inner->crop.error;
-    clx::PackedBuffers& pb = b->packed;
-    pb.T = max_samples;
-    clx::ResampleBuffers& rs = b->rs;
-    rs.n_crops = (uint32_t)max_excerpts;
-    rs.C = (uint32_t)C;
-    rs.L = stride;
-    rs.tile = t.tile;
-    rs.excerpts = const_cast<clx_packed_request*>(inner->packed.requests);
-    rs.count = const_cast<uint32_t*>(inner->packed.count);
-    rs.starts = inner->packed.starts;
-    rs.src = static_cast<const float*>((const void*)inner->buf.conv);
-    rs.src_stride = inner->stride;
-    cudaError_t e = cudaSetDevice(ctx->device);
-    if (e == cudaSuccess) e = device_zeros(pb.requests, max_excerpts);
-    if (e == cudaSuccess) e = device_zeros(pb.count, 1);
-    if (e == cudaSuccess) e = device_zeros(pb.starts, max_excerpts);
-    if (e == cudaSuccess) e = device_zeros(cb.lengths, max_excerpts);
-    if (e == cudaSuccess) e = device_zeros(b->buf.conv, (b->out_elems + 8) * sizeof(float));  // (the slack of fit())
-    if (e == cudaSuccess) e = cudaMalloc((void**)&rs.plan, max_excerpts * sizeof(clx::ResamplePlan));
-    if (e == cudaSuccess) e = upload(rs.file_rate, t.file_rate);
-    if (e == cudaSuccess) e = upload(rs.rates, t.rates);
-    if (e == cudaSuccess) e = upload(rs.coefs, t.coefs);
-    if (e == cudaSuccess) e = upload(rs.k0, t.k0);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
-    if (e != cudaSuccess) {
-        clx_batch_destroy(ctx, b);
-        return cuda_fail(ctx, e, "clx_batch_create_resampled_packed");
-    }
-    rs.lengths = cb.lengths;
-    rs.out = reinterpret_cast<float*>(b->buf.conv);
-    build_graph(ctx, b);
-    *out = b;
+    b->packed.T = max_samples;
+    if (*e == cudaSuccess) *e = fill_resample(b, t, max_excerpts, C, stride);
+    if (*e == cudaSuccess) *e = device_zeros(b, b->packed.requests, max_excerpts);
+    if (*e == cudaSuccess) *e = device_zeros(b, b->packed.count, 1);
+    if (*e == cudaSuccess) *e = device_zeros(b, b->packed.starts, max_excerpts);
     return CLX_OK;
 }
 
-int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
-                               size_t n_crops, size_t num_frames, uint32_t target_rate, const clx_mel_params* params,
-                               const float* window, const float* fbank, clx_batch** out) {
-    if (!out) return CLX_ERR_INVALID_ARGUMENT;
-    *out = nullptr;
+// Mel crop and packed batches: the features of `rows` rows of F frames, `tiles` tiles of frames per row, of the inner
+// batch's output, with the parameters `p` and the tables `t`.  Requests, status, lengths and error word are the inner
+// batch's.
+cudaError_t fill_mel(clx_batch* b, const clx_mel_params* p, const clx::MelTables& t, uint64_t F, size_t rows,
+                     uint64_t tiles) {
+    const clx_batch* inner = b->inner;
+    b->crop = inner->crop;
+    b->mode = CLX_OUT_CHANNELS_F32;
+    b->stride = F;
+    b->out_elems = rows * p->n_mels * F;
+    clx::MelBuffers& mb = b->mel;
+    mb.src = reinterpret_cast<const float*>(inner->buf.conv);
+    mb.L = inner->stride;
+    mb.F = F;
+    mb.rows = (uint32_t)rows;
+    mb.tiles = (uint32_t)tiles;
+    mb.n_fft = p->n_fft;
+    mb.hop = p->hop_length;
+    mb.n_mels = p->n_mels;
+    mb.tile = t.tile;
+    mb.flags = p->flags;
+    mb.log_floor = p->log_floor;
+    mb.log_of_floor = (p->flags & CLX_MEL_LOG) ? (float)std::log((double)p->log_floor) : 0.f;
+    b->mel_smem = t.smem;
+    cudaError_t e = clx::mel_init();
+    if (e == cudaSuccess) e = alloc_output(b);
+    if (e == cudaSuccess) e = upload(b, mb.tw, t.tw);
+    if (e == cudaSuccess) e = upload(b, mb.window, t.window);
+    if (e == cudaSuccess) e = upload(b, mb.bands, t.bands);
+    if (e == cudaSuccess) e = upload(b, mb.weights, t.weights);
+    mb.out = reinterpret_cast<float*>(b->buf.conv);
+    return e;
+}
+
+int make_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files, size_t n_crops,
+                   size_t num_frames, uint32_t target_rate, const clx_mel_params* params, const float* window,
+                   const float* fbank, clx_batch** out, cudaError_t* e) {
     if (!ctx || !corpus || n_crops == 0 || n_crops >= (1u << 30)) return CLX_ERR_INVALID_ARGUMENT;
     clx::MelTables t;
     if (!clx::mel_tables(params, window, fbank, &t)) return CLX_ERR_INVALID_ARGUMENT;
@@ -1471,64 +1426,18 @@ int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t*
     const uint64_t tiles = (F + t.tile - 1) / t.tile;
     if (F > (SIZE_MAX / 4 - 8) / (rows * params->n_mels) || tiles >= (1u << 31) / rows) return CLX_ERR_INVALID_ARGUMENT;
     clx_batch* inner = nullptr;
-    const int rc = target_rate ? clx_batch_create_resampled_crops(ctx, corpus, file_rates, n_files, n_crops, num_frames,
-                                                                  target_rate, &inner)
-                               : clx_batch_create_crops(ctx, corpus, n_crops, num_frames, CLX_OUT_CHANNELS_F32, &inner);
+    const int rc = target_rate ? make_resampled_crops(ctx, corpus, file_rates, n_files, n_crops, num_frames,
+                                                      target_rate, &inner, e)
+                               : make_crops(ctx, corpus, n_crops, num_frames, CLX_OUT_CHANNELS_F32, &inner, e);
     if (rc != CLX_OK) return rc;
-    clx_batch* b = new clx_batch();
-    b->corpus = corpus;
-    corpus->live++;
-    b->inner = inner;
-    b->is_mel = true;
-    b->out_elems = rows * params->n_mels * F;
-    b->mode = CLX_OUT_CHANNELS_F32;
-    b->stride = F;
-    b->crop.requests = inner->crop.requests;
-    b->crop.status = inner->crop.status;
-    b->crop.lengths = inner->crop.lengths;
-    b->crop.error = inner->crop.error;
-    b->crop.n_crops = (uint32_t)n_crops;
-    b->crop.C = (uint32_t)C;
-    b->crop.L = num_frames;
-    clx::MelBuffers& mb = b->mel;
-    mb.src = reinterpret_cast<const float*>(inner->buf.conv);
-    mb.L = num_frames;
-    mb.F = F;
-    mb.rows = (uint32_t)rows;
-    mb.tiles = (uint32_t)tiles;
-    mb.n_fft = params->n_fft;
-    mb.hop = params->hop_length;
-    mb.n_mels = params->n_mels;
-    mb.tile = t.tile;
-    mb.flags = params->flags;
-    mb.log_floor = params->log_floor;
-    mb.log_of_floor = (params->flags & CLX_MEL_LOG) ? (float)std::log((double)params->log_floor) : 0.f;
-    b->mel_smem = t.smem;
-    cudaError_t e = cudaSetDevice(ctx->device);
-    if (e == cudaSuccess) e = clx::mel_init();
-    if (e == cudaSuccess) e = device_zeros(b->buf.conv, (b->out_elems + 8) * sizeof(float));  // (the slack of fit())
-    if (e == cudaSuccess) e = upload(mb.tw, t.tw);
-    if (e == cudaSuccess) e = upload(mb.window, t.window);
-    if (e == cudaSuccess) e = upload(mb.bands, t.bands);
-    if (e == cudaSuccess) e = upload(mb.weights, t.weights);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
-    if (e != cudaSuccess) {
-        clx_batch_destroy(ctx, b);
-        return cuda_fail(ctx, e, "clx_batch_create_mel_crops");
-    }
-    mb.out = reinterpret_cast<float*>(b->buf.conv);
-    build_graph(ctx, b);
-    *out = b;
+    clx_batch* b = *out = new_batch(Kind::MelCrops, corpus, inner);
+    if (*e == cudaSuccess) *e = fill_mel(b, params, t, F, rows, tiles);
     return CLX_OK;
 }
 
-int clx_batch_create_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
-                                size_t max_excerpts, size_t max_samples, uint32_t target_rate,
-                                const clx_mel_params* params, const float* window, const float* fbank,
-                                clx_batch** out) {
-    if (!out) return CLX_ERR_INVALID_ARGUMENT;
-    *out = nullptr;
+int make_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files, size_t max_excerpts,
+                    size_t max_samples, uint32_t target_rate, const clx_mel_params* params, const float* window,
+                    const float* fbank, clx_batch** out, cudaError_t* e) {
     if (!ctx || !corpus || max_excerpts == 0 || max_excerpts >= (1u << 30) || max_samples == 0)
         return CLX_ERR_INVALID_ARGUMENT;
     clx::MelTables t;
@@ -1538,71 +1447,111 @@ int clx_batch_create_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t
     if (F == SIZE_MAX || F > (SIZE_MAX / 4 - 8) / (C * params->n_mels) || tiles >= (1u << 31) / C)
         return CLX_ERR_INVALID_ARGUMENT;
     clx_batch* inner = nullptr;
-    const int rc = target_rate ? clx_batch_create_resampled_packed(ctx, corpus, file_rates, n_files, max_excerpts,
-                                                                   max_samples, target_rate, &inner)
-                               : clx_batch_create_packed(ctx, corpus, max_excerpts, max_samples, CLX_OUT_CHANNELS_F32,
-                                                         &inner);
+    const int rc = target_rate ? make_resampled_packed(ctx, corpus, file_rates, n_files, max_excerpts, max_samples,
+                                                       target_rate, &inner, e)
+                               : make_packed(ctx, corpus, max_excerpts, max_samples, CLX_OUT_CHANNELS_F32, &inner, e);
     if (rc != CLX_OK) return rc;
-    clx_batch* b = new clx_batch();
-    b->corpus = corpus;
-    corpus->live++;
-    b->inner = inner;
-    b->is_mel = true;
-    b->is_packed = true;
-    b->out_elems = C * params->n_mels * F;
-    b->mode = CLX_OUT_CHANNELS_F32;
-    b->stride = F;
-    b->crop.requests = inner->crop.requests;
-    b->crop.status = inner->crop.status;
-    b->crop.lengths = inner->crop.lengths;
-    b->crop.error = inner->crop.error;
-    b->crop.n_crops = (uint32_t)max_excerpts;
-    b->crop.C = (uint32_t)C;
+    clx_batch* b = *out = new_batch(Kind::MelPacked, corpus, inner);
     b->packed.requests = inner->packed.requests;
     b->packed.count = inner->packed.count;
     b->packed.T = max_samples;
-    clx::MelBuffers& mb = b->mel;
-    mb.src = reinterpret_cast<const float*>(inner->buf.conv);
-    mb.L = inner->stride;
-    mb.F = F;
-    mb.rows = (uint32_t)C;
-    mb.tiles = (uint32_t)tiles;
-    mb.n_fft = params->n_fft;
-    mb.hop = params->hop_length;
-    mb.n_mels = params->n_mels;
-    mb.tile = t.tile;
-    mb.flags = params->flags;
-    mb.log_floor = params->log_floor;
-    mb.log_of_floor = (params->flags & CLX_MEL_LOG) ? (float)std::log((double)params->log_floor) : 0.f;
-    b->mel_smem = t.smem;
     clx::MelPacked& mp = b->mel_packed;
     mp.count = inner->packed.count;
     mp.lengths = inner->crop.lengths;
     mp.src_starts = inner->packed.starts;
     mp.n = (uint32_t)max_excerpts;
-    cudaError_t e = cudaSetDevice(ctx->device);
-    if (e == cudaSuccess) e = clx::mel_init();
-    if (e == cudaSuccess) e = device_zeros(b->buf.conv, (b->out_elems + 8) * sizeof(float));  // (the slack of fit())
-    if (e == cudaSuccess) e = device_zeros(b->packed.starts, max_excerpts);
-    if (e == cudaSuccess) e = device_zeros(mp.frames, max_excerpts);
-    if (e == cudaSuccess) e = upload(mb.tw, t.tw);
-    if (e == cudaSuccess) e = upload(mb.window, t.window);
-    if (e == cudaSuccess) e = upload(mb.bands, t.bands);
-    if (e == cudaSuccess) e = upload(mb.weights, t.weights);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_start);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev_stop);
-    if (e != cudaSuccess) {
-        clx_batch_destroy(ctx, b);
-        return cuda_fail(ctx, e, "clx_batch_create_mel_packed");
-    }
+    if (*e == cudaSuccess) *e = fill_mel(b, params, t, F, C, tiles);
+    if (*e == cudaSuccess) *e = device_zeros(b, b->packed.starts, max_excerpts);
+    if (*e == cudaSuccess) *e = device_zeros(b, mp.frames, max_excerpts);
     mp.starts = b->packed.starts;
-    mb.out = reinterpret_cast<float*>(b->buf.conv);
-    build_graph(ctx, b);
-    *out = b;
     return CLX_OK;
 }
 
-void* clx_batch_mel_frames(clx_batch* b) { return b && b->is_mel && b->is_packed ? (void*)b->mel_packed.frames : nullptr; }
+bool corpus_kind(const clx_batch* b) { return b && b->kind != Kind::Frames; }
+bool packed_kind(const clx_batch* b) {
+    return b && (b->kind == Kind::Packed || b->kind == Kind::ResampledPacked || b->kind == Kind::MelPacked);
+}
+}  // namespace
+
+extern "C" {
+
+int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, size_t num_frames, uint32_t mode,
+                           clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    clx_batch* b = nullptr;
+    cudaError_t e = cudaSuccess;
+    const int rc = make_crops(ctx, corpus, n_crops, num_frames, mode, &b, &e);
+    return rc ? rc : finish(ctx, b, e, "clx_batch_create_crops", out);
+}
+
+void* clx_batch_crop_requests(clx_batch* b) { return corpus_kind(b) ? (void*)b->crop.requests : nullptr; }
+void* clx_batch_crop_status(clx_batch* b) { return corpus_kind(b) ? (void*)b->crop.status : nullptr; }
+void* clx_batch_crop_lengths(clx_batch* b) { return corpus_kind(b) ? (void*)b->crop.lengths : nullptr; }
+void* clx_batch_crop_error(clx_batch* b) { return corpus_kind(b) ? (void*)b->crop.error : nullptr; }
+
+int clx_batch_create_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpts, size_t max_samples, uint32_t mode,
+                            clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    clx_batch* b = nullptr;
+    cudaError_t e = cudaSuccess;
+    const int rc = make_packed(ctx, corpus, max_excerpts, max_samples, mode, &b, &e);
+    return rc ? rc : finish(ctx, b, e, "clx_batch_create_packed", out);
+}
+
+void* clx_batch_packed_requests(clx_batch* b) { return packed_kind(b) ? (void*)b->packed.requests : nullptr; }
+void* clx_batch_packed_count(clx_batch* b) { return packed_kind(b) ? (void*)b->packed.count : nullptr; }
+void* clx_batch_packed_starts(clx_batch* b) { return packed_kind(b) ? (void*)b->packed.starts : nullptr; }
+size_t clx_batch_packed_stride(clx_batch* b) { return packed_kind(b) ? b->stride : 0; }
+
+int clx_batch_create_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                                     size_t n_crops, size_t num_frames, uint32_t target_rate, clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    clx_batch* b = nullptr;
+    cudaError_t e = cudaSuccess;
+    const int rc = make_resampled_crops(ctx, corpus, file_rates, n_files, n_crops, num_frames, target_rate, &b, &e);
+    return rc ? rc : finish(ctx, b, e, "clx_batch_create_resampled_crops", out);
+}
+
+int clx_batch_create_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                                      size_t max_excerpts, size_t max_samples, uint32_t target_rate, clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    clx_batch* b = nullptr;
+    cudaError_t e = cudaSuccess;
+    const int rc = make_resampled_packed(ctx, corpus, file_rates, n_files, max_excerpts, max_samples, target_rate, &b,
+                                         &e);
+    return rc ? rc : finish(ctx, b, e, "clx_batch_create_resampled_packed", out);
+}
+
+int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                               size_t n_crops, size_t num_frames, uint32_t target_rate, const clx_mel_params* params,
+                               const float* window, const float* fbank, clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    clx_batch* b = nullptr;
+    cudaError_t e = cudaSuccess;
+    const int rc = make_mel_crops(ctx, corpus, file_rates, n_files, n_crops, num_frames, target_rate, params, window,
+                                  fbank, &b, &e);
+    return rc ? rc : finish(ctx, b, e, "clx_batch_create_mel_crops", out);
+}
+
+int clx_batch_create_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
+                                size_t max_excerpts, size_t max_samples, uint32_t target_rate,
+                                const clx_mel_params* params, const float* window, const float* fbank,
+                                clx_batch** out) {
+    if (!out) return CLX_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    clx_batch* b = nullptr;
+    cudaError_t e = cudaSuccess;
+    const int rc = make_mel_packed(ctx, corpus, file_rates, n_files, max_excerpts, max_samples, target_rate, params,
+                                   window, fbank, &b, &e);
+    return rc ? rc : finish(ctx, b, e, "clx_batch_create_mel_packed", out);
+}
+
+void* clx_batch_mel_frames(clx_batch* b) { return b && b->kind == Kind::MelPacked ? (void*)b->mel_packed.frames : nullptr; }
 
 }  // extern "C"
 

@@ -229,16 +229,15 @@ struct clx_batch {
     uint32_t mode = CLX_OUT_PLANAR_I32;
     uint64_t stride = 0;
     // Corpus batches.  Crops and Packed decode frames of `corpus`: buf.bytes is the corpus's, or over a host corpus the
-    // batch's own staging buffer (span_stride apart per crop, or the staging bound of a packed batch), the filler frame
-    // after it; the planner writes buf.descs, buf.cols and buf.wins in every decode (clx_crops.cu).  The other kinds
-    // wrap `inner`, whose launch sequence runs inside theirs, and write their output to buf.conv.  The buffers below
-    // are the kinds' device state; a wrapper's may point into its inner batch's.  `owned` lists every device allocation
-    // of the batch outside `buf`, which is all clx_batch_destroy frees besides `buf` and `inner`.
+    // batch's own staging buffer of `staging` bytes, the filler frame after it; the planner writes buf.descs, buf.cols
+    // and buf.wins in every decode (clx_crops.cu).  The other kinds wrap `inner`, whose launch sequence runs inside
+    // theirs, and write their output to buf.conv.  The buffers below are the kinds' device state; a wrapper's may point
+    // into its inner batch's.  `owned` lists every device allocation of the batch outside `buf`, which is all
+    // clx_batch_destroy frees besides `buf` and `inner`.
     clx_corpus* corpus = nullptr;
     std::vector<void*> owned;
-    clx::CropBuffers crop{};
-    uint64_t span_stride = 0;
-    clx::PackedBuffers packed{};
+    clx::ExcerptBuffers ex{};
+    uint64_t staging = 0;
     clx_batch* inner = nullptr;
     clx::ResampleBuffers rs{};
     clx::MelBuffers mel{};
@@ -263,9 +262,9 @@ struct clx_corpus {
     std::vector<uint32_t> file_frames;
     uint32_t channels = 1, max_bps = 0;
     int live = 0;  // crop and packed batches of this corpus
-    clx::CropCorpus view(uint64_t span_stride) const {
+    clx::CropCorpus view(uint64_t staging) const {
         return {d_descs, d_starts, d_file_frames, d_file_len, d_file_ch, d_file_tail, n_files, n_frames, d_host,
-                d_host ? span_stride : 0};
+                d_host ? staging : 0};
     }
 };
 
@@ -687,18 +686,19 @@ cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
     case Kind::Frames:
         return clx::launch_decode(db, b->plan, b->device_crc, st, launches);
     case Kind::Crops:
-        return clx::launch_crops(b->corpus->view(b->span_stride), b->crop, db, b->plan, b->device_crc, st, launches);
+        return clx::launch_excerpts<clx::CropLayout>(b->corpus->view(b->staging), b->ex, db, b->plan, b->device_crc, st,
+                                                     launches);
     case Kind::Packed:
-        return clx::launch_packed(b->corpus->view(b->span_stride), b->crop, b->packed, db, b->plan, b->device_crc, st,
-                                  launches);
+        return clx::launch_excerpts<clx::PackedLayout>(b->corpus->view(b->staging), b->ex, db, b->plan, b->device_crc,
+                                                       st, launches);
     case Kind::ResampledCrops:
-        e = clx::launch_resample_map(b->corpus->view(0), b->rs, st, launches);
+        e = clx::launch_resample_map<clx::CropLayout>(b->corpus->view(0), b->rs, b->ex, st, launches);
         if (e == cudaSuccess) e = launch_batch(b->inner, st, launches);
         return e == cudaSuccess ? clx::launch_resample(b->rs, st, launches) : e;
     case Kind::ResampledPacked:
-        e = clx::launch_resample_packed_map(b->corpus->view(0), b->rs, b->packed, st, launches);
+        e = clx::launch_resample_map<clx::PackedLayout>(b->corpus->view(0), b->rs, b->ex, st, launches);
         if (e == cudaSuccess) e = launch_batch(b->inner, st, launches);
-        return e == cudaSuccess ? clx::launch_resample_packed(b->rs, b->packed, st, launches) : e;
+        return e == cudaSuccess ? clx::launch_resample_packed(b->rs, b->ex, st, launches) : e;
     case Kind::MelCrops:
         e = launch_batch(b->inner, st, launches);
         return e == cudaSuccess ? clx::launch_mel(b->mel, b->mel_smem, st, launches) : e;
@@ -1177,29 +1177,30 @@ clx::Plan corpus_plan(const clx_ctx* ctx, const clx_corpus* corpus, size_t* slot
     *slot_elems = ((size_t)plan.max_frame_elems + 3) & ~(size_t)3;
     return plan;
 }
-// The buffers crop and packed batches share, once the kind has set b->crop's sizes and b->span_stride: the frame bytes
-// (the corpus's, or over a host corpus `staged` bytes of staging and then the filler frame), the slots' planar scratch,
-// an output of conv_elems elements (trash included), and the planner's per-excerpt buffers.
-cudaError_t alloc_planned(clx_ctx* ctx, clx_batch* b, const clx::Plan& plan, uint32_t mode, size_t staged,
-                          size_t conv_elems) {
+// The buffers crop and packed batches share, once the kind has set b->ex's sizes and b->staging: the frame bytes (the
+// corpus's, or over a host corpus `staging` bytes of staging and then the filler frame), the slots' planar scratch, an
+// output of conv_elems elements (trash included), and the planner's per-excerpt buffers.
+cudaError_t alloc_planned(clx_ctx* ctx, clx_batch* b, const clx::Plan& plan, uint32_t mode, size_t conv_elems) {
     const clx_corpus* c = b->corpus;
-    clx::CropBuffers& cb = b->crop;
-    const size_t n = cb.n_crops, filler_len = clx::filler_frame(nullptr, 0);
-    b->n_frames = cb.n_slots;
+    clx::ExcerptBuffers& eb = b->ex;
+    const size_t n = eb.n, staged = b->staging, filler_len = clx::filler_frame(nullptr, 0);
+    b->n_frames = eb.n_slots;
     b->plan = plan;
     b->mode = mode;
     b->device_crc = !(ctx->flags & CLX_OPT_NO_VERIFY_CRC);
     if (!c->h_bytes) b->buf.borrow(c->d_bytes, c->buf_bytes);
-    cudaError_t e = b->buf.fit({staged + filler_len, cb.n_slots, cb.n_slots * cb.slot_elems, mode, conv_elems, true, plan},
-                               false);
+    cudaError_t e = b->buf.fit({staged + filler_len, eb.n_slots, (size_t)eb.n_slots * eb.slot_elems, mode, conv_elems,
+                                true, plan}, false);
     if (e == cudaSuccess && c->h_bytes)
         e = cudaMemcpy(b->buf.bytes + staged, c->h_bytes + c->nbytes, filler_len, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = device_zeros(b, cb.status, n);
-    if (e == cudaSuccess) e = device_zeros(b, cb.lengths, n);
-    if (e == cudaSuccess) e = device_alloc(b, cb.error, 1);
-    if (e == cudaSuccess) e = cudaMemset(cb.error, 0xff, sizeof(unsigned long long));
-    if (e == cudaSuccess) e = device_alloc(b, cb.plan, n);
-    if (e == cudaSuccess) e = device_alloc(b, cb.scan, n + 1);
+    if (e == cudaSuccess) e = device_zeros(b, eb.status, n);
+    if (e == cudaSuccess) e = device_zeros(b, eb.lengths, n);
+    if (e == cudaSuccess) e = device_alloc(b, eb.error, 1);
+    if (e == cudaSuccess) e = cudaMemset(eb.error, 0xff, sizeof(unsigned long long));
+    if (e == cudaSuccess) e = device_alloc(b, eb.plan, n);
+    if (e == cudaSuccess) e = device_alloc(b, eb.scan, n + 1);
+    if (e == cudaSuccess) e = device_zeros(b, eb.stage, n);
+    if (e == cudaSuccess) e = device_zeros(b, eb.chunks, n + 1);
     return e;
 }
 
@@ -1217,8 +1218,8 @@ int make_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, size_t num_fram
     if (S == 0 || S > UINT32_MAX / n_crops || num_frames > (SIZE_MAX / 4 - 8) / (rows + C)) return CLX_ERR_INVALID_ARGUMENT;
     const size_t slots = n_crops * S;
     if (slots > (SIZE_MAX / 4 - 8) / slot_elems) return CLX_ERR_INVALID_ARGUMENT;
-    // Over a host corpus, the batch's own frame bytes: crop b's span at b * span_stride + (its start & 15), then the
-    // filler frame after the last span.
+    // Over a host corpus, the batch's own frame bytes: room for n_crops spans of the bytes bound + 15, each rounded up
+    // to 16 (the spans are packed from 0 by the planner), then the filler frame.
     size_t span_stride = 0;
     if (corpus->h_bytes) {
         const size_t span = clx_crop_bytes_bound(corpus->descs.data(), corpus->n_frames, corpus->file_frames.data(),
@@ -1228,19 +1229,18 @@ int make_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, size_t num_fram
     }
     CU(ctx, cudaSetDevice(ctx->device));
     clx_batch* b = *out = new_batch(Kind::Crops, corpus);
-    b->span_stride = span_stride;
+    b->staging = n_crops * span_stride;
     b->out_elems = rows * num_frames;
     b->stride = num_frames;
-    clx::CropBuffers& cb = b->crop;
-    cb.n_crops = (uint32_t)n_crops;
-    cb.C = (uint32_t)C;
-    cb.S = (uint32_t)S;
-    cb.n_slots = (uint32_t)slots;
-    cb.L = num_frames;
-    cb.slot_elems = slot_elems;
+    clx::ExcerptBuffers& eb = b->ex;
+    eb.n = (uint32_t)n_crops;
+    eb.C = (uint32_t)C;
+    eb.n_slots = (uint32_t)slots;
+    eb.L = num_frames;
+    eb.slot_elems = (uint32_t)slot_elems;
     // the output plus C trash rows for the unused slots
-    *e = alloc_planned(ctx, b, plan, mode, n_crops * span_stride, (rows + C) * num_frames);
-    if (*e == cudaSuccess) *e = device_zeros(b, cb.requests, n_crops);
+    *e = alloc_planned(ctx, b, plan, mode, (rows + C) * num_frames);
+    if (*e == cudaSuccess) *e = device_zeros(b, eb.crop_requests, n_crops);
     return CLX_OK;
 }
 
@@ -1262,36 +1262,29 @@ int make_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpts, size_t ma
         return CLX_ERR_INVALID_ARGUMENT;
     // Over a host corpus, the batch's own frame bytes: the excerpts' spans packed from 0 (at most the bytes bound), then
     // the filler frame.
-    size_t span_stride = 0, chunks = 0;
+    size_t staging = 0;
     if (corpus->h_bytes) {
-        span_stride = clx_packed_bytes_bound(descs, corpus->n_frames, ff, corpus->n_files, max_excerpts, max_samples);
-        if (span_stride > SIZE_MAX / 2) return CLX_ERR_INVALID_ARGUMENT;
-        chunks = span_stride / (16 * 1024) + max_excerpts;  // ceil(span / GATHER_CHUNK) per excerpt, every span together
+        staging = clx_packed_bytes_bound(descs, corpus->n_frames, ff, corpus->n_files, max_excerpts, max_samples);
+        if (staging > SIZE_MAX / 2) return CLX_ERR_INVALID_ARGUMENT;
     }
     CU(ctx, cudaSetDevice(ctx->device));
     clx_batch* b = *out = new_batch(Kind::Packed, corpus);
-    b->span_stride = span_stride;
+    b->staging = staging;
     b->out_elems = C * stride;
     b->stride = stride;
-    clx::CropBuffers& cb = b->crop;
-    cb.n_crops = (uint32_t)max_excerpts;
-    cb.C = (uint32_t)C;
-    cb.S = (uint32_t)S;
-    cb.n_slots = (uint32_t)S;
-    cb.L = stride;
-    cb.slot_elems = slot_elems;
-    clx::PackedBuffers& pb = b->packed;
-    pb.T = max_samples;
-    pb.W = W;
-    pb.max_chunks = (uint32_t)std::min<size_t>(std::max<size_t>(chunks, 1), 1u << 20);
+    clx::ExcerptBuffers& eb = b->ex;
+    eb.n = (uint32_t)max_excerpts;
+    eb.C = (uint32_t)C;
+    eb.n_slots = (uint32_t)S;
+    eb.L = stride;
+    eb.T = max_samples;
+    eb.slot_elems = (uint32_t)slot_elems;
     // the output with its trash columns, zeroed here: afterwards every call zeroes what it must
-    *e = alloc_planned(ctx, b, plan, mode, span_stride, C * stride);
-    if (*e == cudaSuccess) *e = device_zeros(b, pb.requests, max_excerpts);
-    if (*e == cudaSuccess) *e = device_zeros(b, pb.count, 1);
-    if (*e == cudaSuccess) *e = device_zeros(b, pb.starts, max_excerpts);
-    if (*e == cudaSuccess) *e = device_zeros(b, pb.stage, max_excerpts);
-    if (*e == cudaSuccess) *e = device_zeros(b, pb.chunks, max_excerpts + 1);
-    if (*e == cudaSuccess) *e = device_zeros(b, pb.end, 2);
+    *e = alloc_planned(ctx, b, plan, mode, C * stride);
+    if (*e == cudaSuccess) *e = device_zeros(b, eb.packed_requests, max_excerpts);
+    if (*e == cudaSuccess) *e = device_zeros(b, eb.count, 1);
+    if (*e == cudaSuccess) *e = device_zeros(b, eb.starts, max_excerpts);
+    if (*e == cudaSuccess) *e = device_zeros(b, eb.end, 2);
     return CLX_OK;
 }
 
@@ -1302,30 +1295,30 @@ cudaError_t fill_resample(clx_batch* b, const clx::ResampleTables& t, size_t n, 
     const clx_batch* inner = b->inner;
     b->mode = CLX_OUT_CHANNELS_F32;
     b->stride = L;
-    clx::CropBuffers& cb = b->crop;
-    cb.n_crops = (uint32_t)n;
-    cb.C = (uint32_t)C;
-    cb.L = L;
-    cb.status = inner->crop.status;
-    cb.error = inner->crop.error;
+    clx::ExcerptBuffers& eb = b->ex;
+    eb.n = (uint32_t)n;
+    eb.C = (uint32_t)C;
+    eb.L = L;
+    eb.status = inner->ex.status;
+    eb.error = inner->ex.error;
     clx::ResampleBuffers& rs = b->rs;
     rs.n_crops = (uint32_t)n;
     rs.C = (uint32_t)C;
     rs.L = L;
     rs.tile = t.tile;
-    rs.excerpts = const_cast<clx_packed_request*>(inner->packed.requests);
-    rs.count = const_cast<uint32_t*>(inner->packed.count);
-    rs.starts = inner->packed.starts;
+    rs.excerpts = const_cast<clx_packed_request*>(inner->ex.packed_requests);
+    rs.count = const_cast<uint32_t*>(inner->ex.count);
+    rs.starts = inner->ex.starts;
     rs.src = static_cast<const float*>((const void*)inner->buf.conv);
     rs.src_stride = inner->stride;
-    cudaError_t e = device_zeros(b, cb.lengths, n);
+    cudaError_t e = device_zeros(b, eb.lengths, n);
     if (e == cudaSuccess) e = alloc_output(b);
     if (e == cudaSuccess) e = device_alloc(b, rs.plan, n);
     if (e == cudaSuccess) e = upload(b, rs.file_rate, t.file_rate);
     if (e == cudaSuccess) e = upload(b, rs.rates, t.rates);
     if (e == cudaSuccess) e = upload(b, rs.coefs, t.coefs);
     if (e == cudaSuccess) e = upload(b, rs.k0, t.k0);
-    rs.lengths = cb.lengths;
+    rs.lengths = eb.lengths;
     rs.out = reinterpret_cast<float*>(b->buf.conv);
     return e;
 }
@@ -1349,8 +1342,7 @@ int make_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_
     clx_batch* b = *out = new_batch(Kind::ResampledCrops, corpus, inner);
     b->out_elems = rows * num_frames;
     if (*e == cudaSuccess) *e = fill_resample(b, t, n_crops, C, num_frames);
-    if (*e == cudaSuccess) *e = device_zeros(b, b->crop.requests, n_crops);
-    b->rs.requests = b->crop.requests;
+    if (*e == cudaSuccess) *e = device_zeros(b, b->ex.crop_requests, n_crops);
     return CLX_OK;
 }
 
@@ -1372,11 +1364,11 @@ int make_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file
     if (rc != CLX_OK) return rc;
     clx_batch* b = *out = new_batch(Kind::ResampledPacked, corpus, inner);
     b->out_elems = C * stride;
-    b->packed.T = max_samples;
+    b->ex.T = max_samples;
     if (*e == cudaSuccess) *e = fill_resample(b, t, max_excerpts, C, stride);
-    if (*e == cudaSuccess) *e = device_zeros(b, b->packed.requests, max_excerpts);
-    if (*e == cudaSuccess) *e = device_zeros(b, b->packed.count, 1);
-    if (*e == cudaSuccess) *e = device_zeros(b, b->packed.starts, max_excerpts);
+    if (*e == cudaSuccess) *e = device_zeros(b, b->ex.packed_requests, max_excerpts);
+    if (*e == cudaSuccess) *e = device_zeros(b, b->ex.count, 1);
+    if (*e == cudaSuccess) *e = device_zeros(b, b->ex.starts, max_excerpts);
     return CLX_OK;
 }
 
@@ -1386,7 +1378,7 @@ int make_resampled_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file
 cudaError_t fill_mel(clx_batch* b, const clx_mel_params* p, const clx::MelTables& t, uint64_t F, size_t rows,
                      uint64_t tiles) {
     const clx_batch* inner = b->inner;
-    b->crop = inner->crop;
+    b->ex = inner->ex;
     b->mode = CLX_OUT_CHANNELS_F32;
     b->stride = F;
     b->out_elems = rows * p->n_mels * F;
@@ -1452,18 +1444,15 @@ int make_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates
                                : make_packed(ctx, corpus, max_excerpts, max_samples, CLX_OUT_CHANNELS_F32, &inner, e);
     if (rc != CLX_OK) return rc;
     clx_batch* b = *out = new_batch(Kind::MelPacked, corpus, inner);
-    b->packed.requests = inner->packed.requests;
-    b->packed.count = inner->packed.count;
-    b->packed.T = max_samples;
     clx::MelPacked& mp = b->mel_packed;
-    mp.count = inner->packed.count;
-    mp.lengths = inner->crop.lengths;
-    mp.src_starts = inner->packed.starts;
+    mp.count = inner->ex.count;
+    mp.lengths = inner->ex.lengths;
+    mp.src_starts = inner->ex.starts;
     mp.n = (uint32_t)max_excerpts;
-    if (*e == cudaSuccess) *e = fill_mel(b, params, t, F, C, tiles);
-    if (*e == cudaSuccess) *e = device_zeros(b, b->packed.starts, max_excerpts);
+    if (*e == cudaSuccess) *e = fill_mel(b, params, t, F, C, tiles);  // b->ex: the inner batch's, but for the starts
+    if (*e == cudaSuccess) *e = device_zeros(b, b->ex.starts, max_excerpts);
     if (*e == cudaSuccess) *e = device_zeros(b, mp.frames, max_excerpts);
-    mp.starts = b->packed.starts;
+    mp.starts = b->ex.starts;
     return CLX_OK;
 }
 
@@ -1485,10 +1474,10 @@ int clx_batch_create_crops(clx_ctx* ctx, clx_corpus* corpus, size_t n_crops, siz
     return rc ? rc : finish(ctx, b, e, "clx_batch_create_crops", out);
 }
 
-void* clx_batch_crop_requests(clx_batch* b) { return corpus_kind(b) ? (void*)b->crop.requests : nullptr; }
-void* clx_batch_crop_status(clx_batch* b) { return corpus_kind(b) ? (void*)b->crop.status : nullptr; }
-void* clx_batch_crop_lengths(clx_batch* b) { return corpus_kind(b) ? (void*)b->crop.lengths : nullptr; }
-void* clx_batch_crop_error(clx_batch* b) { return corpus_kind(b) ? (void*)b->crop.error : nullptr; }
+void* clx_batch_crop_requests(clx_batch* b) { return corpus_kind(b) ? (void*)b->ex.crop_requests : nullptr; }
+void* clx_batch_crop_status(clx_batch* b) { return corpus_kind(b) ? (void*)b->ex.status : nullptr; }
+void* clx_batch_crop_lengths(clx_batch* b) { return corpus_kind(b) ? (void*)b->ex.lengths : nullptr; }
+void* clx_batch_crop_error(clx_batch* b) { return corpus_kind(b) ? (void*)b->ex.error : nullptr; }
 
 int clx_batch_create_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpts, size_t max_samples, uint32_t mode,
                             clx_batch** out) {
@@ -1500,9 +1489,9 @@ int clx_batch_create_packed(clx_ctx* ctx, clx_corpus* corpus, size_t max_excerpt
     return rc ? rc : finish(ctx, b, e, "clx_batch_create_packed", out);
 }
 
-void* clx_batch_packed_requests(clx_batch* b) { return packed_kind(b) ? (void*)b->packed.requests : nullptr; }
-void* clx_batch_packed_count(clx_batch* b) { return packed_kind(b) ? (void*)b->packed.count : nullptr; }
-void* clx_batch_packed_starts(clx_batch* b) { return packed_kind(b) ? (void*)b->packed.starts : nullptr; }
+void* clx_batch_packed_requests(clx_batch* b) { return packed_kind(b) ? (void*)b->ex.packed_requests : nullptr; }
+void* clx_batch_packed_count(clx_batch* b) { return packed_kind(b) ? (void*)b->ex.count : nullptr; }
+void* clx_batch_packed_starts(clx_batch* b) { return packed_kind(b) ? (void*)b->ex.starts : nullptr; }
 size_t clx_batch_packed_stride(clx_batch* b) { return packed_kind(b) ? b->stride : 0; }
 
 int clx_batch_create_resampled_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,

@@ -93,11 +93,11 @@ cudaError_t launch_channels(const clx_frame_desc* d_descs, uint32_t n_frames, ui
 // mark[f] = (results[f].status == status) for every frame, unless *gate == 0 (then nothing is written).
 cudaError_t launch_mark_status(const clx_frame_result* d_results, uint32_t n_frames, int32_t status, uint8_t* d_mark,
                                const int* gate, cudaStream_t stream, uint64_t* launches);
-// clx_crops.cu: crop batches.  A corpus on the device: its descriptors (descs[n_frames] is the filler frame), each
-// frame's first sample within its file, each file's frame range [file_frames[i], file_frames[i + 1]), length, channel
-// count and trailing-bytes verdict.  A corpus in host memory (CLX_CORPUS_HOST) also gives the device address of its
-// mapped pinned bytes and the batch's span stride: each call gathers crop b's span of frames into the batch's staging
-// buffer at b * span_stride + (span start & 15), and the descriptors point there.  Both are 0 for a device corpus.
+// clx_crops.cu: crop and packed batches.  A corpus on the device: its descriptors (descs[n_frames] is the filler frame),
+// each frame's first sample within its file, each file's frame range [file_frames[i], file_frames[i + 1]), length,
+// channel count and trailing-bytes verdict.  A corpus in host memory (CLX_CORPUS_HOST) also gives the device address of
+// its mapped pinned bytes and the size of the batch's staging buffer: each call gathers the excerpts' spans of frames
+// into it, the filler frame follows at `staging`, and the descriptors point there.  Both are 0 for a device corpus.
 struct CropCorpus {
     const clx_frame_desc* descs;
     const int64_t* starts;
@@ -107,42 +107,44 @@ struct CropCorpus {
     const int32_t* file_tail;
     uint32_t n_files, n_frames;
     const uint8_t* host_bytes;
-    uint64_t span_stride;
+    uint64_t staging;
 };
-// Per crop, what the planner found (device memory, written every decode).
-struct CropPlan {
+// Per excerpt, what the planner found (device memory, written every decode).
+struct ExcerptPlan {
     int64_t lo;       // first sample of the excerpt
     uint32_t count;   // frames overlapping it
     uint32_t first;   // corpus index of the first of them
     uint32_t file;
     uint32_t ch;      // rows the excerpt covers (0: an invalid request)
 };
-struct CropBuffers {
-    const clx_crop_request* requests;
+// The excerpts of a crop or packed batch (and the requests, lengths and layout of a resampled one).  A crop batch is
+// a packed batch whose excerpts each own a row group: where an excerpt's output starts, whether it fits and what is
+// zeroed around it is the layout's (CropLayout, PackedLayout in clx_scan.cuh), everything else is shared.  Over a host
+// corpus the staging buffer holds each excerpt's span at stage[b], the scan of span bytes + 15 moved up to the span
+// start's residue mod 16.
+struct ExcerptBuffers {
+    const clx_crop_request* crop_requests;      // crop batches: n requests, length L
+    const clx_packed_request* packed_requests;  // packed batches: n requests ...
+    const uint32_t* count;                      // ... of which this call uses the first *count (device, by the caller)
     int32_t* status;
     int64_t* lengths;
     unsigned long long* error;
-    CropPlan* plan;
-    uint32_t* scan;   // n_crops + 1: exclusive scan of the counts, then the total
-    uint32_t n_crops, C, S, n_slots;
-    uint64_t L;       // num_frames: the row length
-    uint64_t slot_elems;
+    ExcerptPlan* plan;
+    uint32_t* scan;   // n + 1: exclusive scan of the slots, then the total
+    int64_t* starts;  // packed batches: each excerpt's first column
+    uint64_t* stage;  // host corpus: where each excerpt's span starts in the staging buffer
+    uint32_t* chunks; // n + 1: exclusive scan of each span's gather chunks, then the total
+    uint64_t* end;    // packed batches: [0] this call's end column, [1] the previous call's
+    uint32_t n, C, n_slots;
+    uint32_t slot_elems;
+    uint64_t L;       // the row length: num_frames of a crop batch, the stride of a packed one (trash columns included)
+    uint64_t T;       // packed batches: max_samples, the columns users see
 };
-// Packed batches (clx_batch_create_packed) keep their per-excerpt plan, status, lengths, error word and slot scan in a
-// CropBuffers (n_crops = max_excerpts, S = n_slots = the slot bound, L = the row stride), and the rest here.  Over a
-// host corpus the staging buffer holds each excerpt's span at stage[b], the scan of span bytes + 15 moved up to the
-// span start's residue mod 16, and the filler frame at CropCorpus::span_stride (the staging bound).
-struct PackedBuffers {
-    const clx_packed_request* requests;
-    const uint32_t* count;  // excerpts this call uses (device, written by the caller)
-    int64_t* starts;        // each excerpt's first column
-    uint64_t* stage;        // host corpus: where each excerpt's span starts in the staging buffer
-    uint32_t* chunks;       // n + 1: exclusive scan of each span's gather chunks, then the total
-    uint64_t* end;          // [0]: this call's end column, [1]: the previous call's
-    uint64_t T;             // max_samples: the columns users see
-    uint64_t W;             // trash columns after round_up_4(T)
-    uint32_t max_chunks;    // the gather's grid
-};
+// Kernels take it by value.  Above 128 bytes nvcc reads such a parameter through a pointer, which took the gather's
+// per-excerpt values off the uniform datapath (40 registers instead of 32).
+static_assert(sizeof(ExcerptBuffers) <= 128, "ExcerptBuffers is a kernel parameter of at most 128 bytes");
+struct CropLayout;
+struct PackedLayout;
 // Filler frame: 1 channel, 16 bits, block size 192, CONSTANT 0.  Writes it if cap suffices; returns its length.
 size_t filler_frame(uint8_t* out, size_t cap);
 // clx_api.cu, for corpus images (clx_corpus_image.cpp): the size of a frame-bytes buffer of `nbytes` bytes (whole
@@ -161,14 +163,13 @@ struct ImageIndex {
 };
 // CLX_OK with `ix` filled, or CLX_ERR_INVALID_ARGUMENT (clx_corpus_image_check's verdict).
 int read_image(const void* image, size_t image_bytes, ImageIndex* ix);
-// The crop batch's launch sequence: planner (count, scan, the gather of a host corpus, emit, zero-fill), launch_decode
-// over every slot, status pass.  `db`: the batch's buffers; db.descs / db.cols / db.wins are written by the planner, and
-// over a host corpus db.bytes is the staging buffer the gather writes.
-cudaError_t launch_crops(const CropCorpus& cc, const CropBuffers& cb, const DecodeBuffers& db, const Plan& plan, bool crc,
-                         cudaStream_t stream, uint64_t* launches);
-// The packed batch's launch sequence, of the same shape (clx_crops.cu).
-cudaError_t launch_packed(const CropCorpus& cc, const CropBuffers& cb, const PackedBuffers& pb, const DecodeBuffers& db,
-                          const Plan& plan, bool crc, cudaStream_t stream, uint64_t* launches);
+// The launch sequence of a crop (Layout = CropLayout) or packed batch (PackedLayout): planner (count, scan, the gather
+// of a host corpus, emit, zero-fill), launch_decode over every slot, status pass.  `db`: the batch's buffers;
+// db.descs / db.cols / db.wins are written by the planner, and over a host corpus db.bytes is the staging buffer the
+// gather writes.
+template <class Layout>
+cudaError_t launch_excerpts(const CropCorpus& cc, const ExcerptBuffers& eb, const DecodeBuffers& db, const Plan& plan,
+                            bool crc, cudaStream_t stream, uint64_t* launches);
 
 // clx_resample.cu: resampled crop batches (clx_batch_create_resampled_crops), a packed batch of each crop's source span
 // between two kernels.  One polyphase table per distinct source rate r != R: with g = gcd(r, R), o = r / g, n = R / g,
@@ -186,7 +187,6 @@ struct ResamplePlan {
     uint32_t ch;               // rows the crop covers (0: an invalid request)
 };
 struct ResampleBuffers {
-    const clx_crop_request* requests;
     int64_t* lengths;               // at rate R
     ResamplePlan* plan;
     const uint32_t* file_rate;      // per file, its ResampleRate
@@ -214,17 +214,18 @@ struct ResampleTables {
     uint32_t tile = 0;
 };
 bool resample_tables(const uint32_t* file_rates, size_t n_files, uint32_t target, size_t num_frames, ResampleTables* t);
-// The two kernels around the packed batch's launch sequence.
-cudaError_t launch_resample_map(const CropCorpus& cc, const ResampleBuffers& rs, cudaStream_t stream, uint64_t* launches);
+// The map kernel before the inner packed batch's launch sequence, of a resampled crop (Layout = CropLayout) or packed
+// batch (PackedLayout): `eb` holds the batch's own requests at rate R (and count, target column starts and T of a
+// packed one).  Then the filter kernel of a crop batch.
+template <class Layout>
+cudaError_t launch_resample_map(const CropCorpus& cc, const ResampleBuffers& rs, const ExcerptBuffers& eb,
+                                cudaStream_t stream, uint64_t* launches);
 cudaError_t launch_resample(const ResampleBuffers& rs, cudaStream_t stream, uint64_t* launches);
 // Resampled packed batches (clx_batch_create_resampled_packed) keep the same ResampleBuffers, with n_crops =
-// max_excerpts, L = the output's row stride and lengths at rate R, and their own PackedBuffers: the caller's requests
-// and count at rate R, the target column starts and T.  The inner packed batch has resample_packed_bound columns
-// (clx_resample_packed_source_bound over t's rates).
+// max_excerpts, L = the output's row stride and lengths at rate R.  The inner packed batch has resample_packed_bound
+// columns (clx_resample_packed_source_bound over t's rates).
 size_t resample_packed_bound(const ResampleTables& t, size_t max_excerpts, size_t max_samples);
-cudaError_t launch_resample_packed_map(const CropCorpus& cc, const ResampleBuffers& rs, const PackedBuffers& pb,
-                                       cudaStream_t stream, uint64_t* launches);
-cudaError_t launch_resample_packed(const ResampleBuffers& rs, const PackedBuffers& pb, cudaStream_t stream,
+cudaError_t launch_resample_packed(const ResampleBuffers& rs, const ExcerptBuffers& eb, cudaStream_t stream,
                                    uint64_t* launches);
 
 // clx_mel.cu: mel crop batches (clx_batch_create_mel_crops), one kernel after an inner crop or resampled crop batch.

@@ -2,16 +2,18 @@
 // a corpus whose files have different sample rates, all at one target rate R, built around an unchanged packed batch.
 //
 // The graph:
-//   1. resample_map_kernel: per crop, validate the request in target terms and write the source span its outputs read,
-//      clipped to the file, as request b of the inner packed batch (an invalid request as an invalid packed request, so
-//      the packed batch's status and error word come out in crop order; an empty crop as the empty excerpt at N).
-//   2. clx::launch_packed of the inner batch, as is: every span decoded to f32 along the columns of its [C, T] output.
+//   1. resample_map_kernel<CropLayout>: per crop, validate the request in target terms and write the source span its
+//      outputs read, clipped to the file, as request b of the inner packed batch (an invalid request as an invalid
+//      packed request, so the packed batch's status and error word come out in crop order; an empty crop as the empty
+//      excerpt at N).
+//   2. clx::launch_excerpts<PackedLayout> of the inner batch, as is: every span decoded to f32 along the columns of its
+//      [C, T] output.
 //   3. resample_kernel: per (tile of outputs, crop, row), the tile's source samples staged in shared memory from the
 //      packed output, then each output the dot product of its phase's coefficients with them.  Writes every element of
 //      [n_crops * C, L], zeros included.
 // Resampled packed batches (clx_batch_create_resampled_packed) have the same graph over excerpts laid out along the
-// columns of one [C, round_up_4(T)] output at rate R: resample_packed_map_kernel (the layout, the fit and the source
-// spans), the inner packed batch, and resample_packed_kernel, which runs resample_kernel's per-tile body on each
+// columns of one [C, round_up_4(T)] output at rate R: resample_map_kernel<PackedLayout> (the layout, the fit and the
+// source spans), the inner packed batch, and resample_packed_kernel, which runs resample_kernel's per-tile body on each
 // excerpt's part of a tile of columns (CLX_RESAMPLE_TILE).
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -26,7 +28,6 @@
 
 namespace clx {
 
-constexpr uint32_t RS_MAP_THREADS = 256;
 constexpr uint32_t RS_THREADS = 256;
 constexpr uint32_t RS_SMEM = 8192;      // source samples a CTA stages (32 KB)
 constexpr uint32_t RS_MAX_TILE = 1024;  // outputs per CTA, 4 per thread
@@ -47,42 +48,62 @@ __device__ __forceinline__ void source_span(const ResampleRate& t, int64_t N, in
     }
 }
 
-__global__ void __launch_bounds__(RS_MAP_THREADS)
-resample_map_kernel(CropCorpus cc, ResampleBuffers rs) {
-    const uint32_t b = blockIdx.x * RS_MAP_THREADS + threadIdx.x;
-    if (b == 0) *rs.count = rs.n_crops;
-    if (b >= rs.n_crops) return;
-    const clx_crop_request r = rs.requests[b];
-    clx_packed_request q{0, 1, 0, 1};  // invalid (reserved != 0): status CLX_ERR_INVALID_ARGUMENT, nothing decoded
-    ResamplePlan p{r.offset, 0, 0, 0, 0};
-    int64_t len = 0;
-    // Requests come from outside the program: nothing is read on behalf of one before it is known to be in range.
-    if (r.reserved == 0 && r.file < cc.n_files && r.offset >= 0) {
-        const uint32_t ti = rs.file_rate[r.file];
-        const ResampleRate t = rs.rates[ti];
-        const int64_t N = cc.file_len[r.file];
-        const int64_t Nt = t.taps ? (int64_t)(((uint64_t)N * t.n + t.o - 1) / t.o) : N;  // (N < 2^36, n < 2^20)
-        if (r.offset <= Nt) {
-            len = (uint64_t)(Nt - r.offset) < rs.L ? Nt - r.offset : (int64_t)rs.L;
-            p.rate = ti;
-            p.ch = cc.file_ch[r.file];
+// One CTA, SCAN_THREADS excerpts at a time: each request validated at rate R (N_t = ceil(N * n / o) in place of N) and
+// its n_b taken, then the layout's start and fit (a packed batch's start_b is the scan of round_up_4(n_b) over the valid
+// excerpts, and an excerpt fits when start_b + n_b <= T; a crop always fits).  One that fits becomes the packed request
+// of its source span (an empty one, offset N_t, the valid empty excerpt at N); one that is invalid or does not fit
+// becomes an invalid packed request in the same position, so the inner batch's status and error word come out in
+// excerpt order, and a non-fit at R cannot reach the inner batch.
+template <class Layout>
+__global__ void __launch_bounds__(SCAN_THREADS)
+resample_map_kernel(CropCorpus cc, ResampleBuffers rs, ExcerptBuffers eb) {
+    __shared__ PackedSums s_warp[SCAN_THREADS / 32];
+    __shared__ PackedSums s_cols;
+    if (threadIdx.x == 0) s_cols = PackedSums{};
+    __syncthreads();
+    const Layout at{eb};
+    const uint32_t n = eb.n, used = at.used();
+    if (threadIdx.x == 0) *rs.count = used;
+    for (uint32_t base = 0; base < n; base += SCAN_THREADS) {
+        const uint32_t i = base + threadIdx.x;
+        clx_packed_request r{0, 1, 0, 1};
+        ResampleRate t{};
+        int64_t N = 0, len = 0;
+        bool valid = false;
+        if (i < n && i < used) {  // (later excerpts are unused: length 0, an unused packed request)
+            r = at.request(i);
+            if (request_ok(r, cc.n_files)) {
+                t = rs.rates[rs.file_rate[r.file]];
+                N = cc.file_len[r.file];
+                const int64_t Nt = t.taps ? (int64_t)(((uint64_t)N * t.n + t.o - 1) / t.o) : N;  // (N < 2^36, n < 2^20)
+                len = excerpt_length(r, Nt);
+                valid = len >= 0;
+                if (!valid) len = 0;
+            }
+        }
+        const uint64_t start = at.start(i, len, s_warp, &s_cols);
+        const bool fit = valid && at.fits(start, len);
+        clx_packed_request q{0, 1, 0, 1};  // invalid (reserved != 0): status CLX_ERR_INVALID_ARGUMENT, nothing decoded
+        ResamplePlan p{0, 0, 0, 0, 0};
+        if (fit) {
             int64_t lo, hi;
             source_span(t, N, r.offset, len, &lo, &hi);
             q = clx_packed_request{r.file, 0, lo, len > 0 ? hi - lo : -1};
-            p.src_lo = lo;
-            p.src_len = hi - lo;
+            p = ResamplePlan{r.offset, lo, hi - lo, rs.file_rate[r.file], cc.file_ch[r.file]};
+        }
+        if (i < n) {
+            rs.lengths[i] = fit ? len : 0;
+            rs.plan[i] = p;
+            rs.excerpts[i] = q;
         }
     }
-    rs.excerpts[b] = q;
-    rs.plan[b] = p;
-    rs.lengths[b] = len;
 }
 
 // Outputs [j0, j0 + m) of one row of a crop or excerpt whose file has rate r != R, into row[j0 ..]: m <= the tile,
 // p its ResamplePlan (offset: output 0's place in the file's resampled signal, src_lo / src_len: the decoded span), t
 // its ResampleRate, x the span's row in the packed output; s_x the CTA's RS_SMEM floats of shared memory.  Every thread
-// of the CTA runs it with the same arguments.  A macro rather than a function, as CLX_GATHER_SPAN in clx_crops.cu: that
-// way resample_kernel compiles exactly as it did with the body written out, and resample_packed_kernel runs the same.
+// of the CTA runs it with the same arguments.  A macro rather than a function: that way resample_kernel compiles exactly
+// as it did with the body written out, and resample_packed_kernel runs the same.
 #define CLX_RESAMPLE_TILE(rs, t, p, x, row, j0, m, s_x)                                                                 \
     do {                                                                                                                \
         const float* coefs = rs.coefs + t.coef;                                                                         \
@@ -158,11 +179,17 @@ resample_kernel(ResampleBuffers rs) {
     }
 }
 
-cudaError_t launch_resample_map(const CropCorpus& cc, const ResampleBuffers& rs, cudaStream_t stream, uint64_t* launches) {
-    resample_map_kernel<<<(rs.n_crops + RS_MAP_THREADS - 1) / RS_MAP_THREADS, RS_MAP_THREADS, 0, stream>>>(cc, rs);
+template <class Layout>
+cudaError_t launch_resample_map(const CropCorpus& cc, const ResampleBuffers& rs, const ExcerptBuffers& eb,
+                                cudaStream_t stream, uint64_t* launches) {
+    resample_map_kernel<Layout><<<1, SCAN_THREADS, 0, stream>>>(cc, rs, eb);
     (*launches)++;
     return cudaGetLastError();
 }
+template cudaError_t launch_resample_map<CropLayout>(const CropCorpus&, const ResampleBuffers&, const ExcerptBuffers&,
+                                                     cudaStream_t, uint64_t*);
+template cudaError_t launch_resample_map<PackedLayout>(const CropCorpus&, const ResampleBuffers&, const ExcerptBuffers&,
+                                                       cudaStream_t, uint64_t*);
 
 cudaError_t launch_resample(const ResampleBuffers& rs, cudaStream_t stream, uint64_t* launches) {
     const dim3 grid((uint32_t)((rs.L + rs.tile - 1) / rs.tile), std::min<uint32_t>(rs.n_crops, 65535), rs.C);
@@ -173,60 +200,7 @@ cudaError_t launch_resample(const ResampleBuffers& rs, cudaStream_t stream, uint
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Resampled packed batches (clx_batch_create_resampled_packed): rs as for crops, with n_crops = max_excerpts and L = the
-// output's row stride; pb holds the caller's requests and count at rate R, and the target column starts.
-
-// One CTA, SCAN_THREADS excerpts at a time, as packed_scan_kernel: each request validated at rate R (N_t = ceil(N * n /
-// o) in place of N) and its n_b taken; start_b is the scan of round_up_4(n_b) over the valid excerpts, and an excerpt
-// fits when start_b + n_b <= T.  One that fits becomes the packed request of its source span, as in
-// resample_map_kernel; one that is invalid or does not fit becomes an invalid packed request in the same position, so
-// the inner batch's status and error word come out in excerpt order, and a non-fit at R cannot reach the inner batch.
-__global__ void __launch_bounds__(SCAN_THREADS)
-resample_packed_map_kernel(CropCorpus cc, ResampleBuffers rs, PackedBuffers pb) {
-    __shared__ PackedSums s_warp[SCAN_THREADS / 32];
-    __shared__ PackedSums s_cols;
-    if (threadIdx.x == 0) s_cols = PackedSums{};
-    __syncthreads();
-    const uint32_t n = rs.n_crops, used = *pb.count;
-    if (threadIdx.x == 0) *rs.count = used;
-    for (uint32_t base = 0; base < n; base += SCAN_THREADS) {
-        const uint32_t i = base + threadIdx.x;
-        clx_packed_request r{0, 1, 0, 1};
-        ResampleRate t{};
-        int64_t N = 0, len = 0;
-        bool valid = false;
-        // Requests come from outside the program: nothing is read on behalf of one before it is known to be in range.
-        if (i < n && i < used) {  // (later excerpts are unused: length 0, an unused packed request)
-            r = pb.requests[i];
-            if (r.reserved == 0 && r.file < cc.n_files && r.offset >= 0 && r.length != 0 && r.length >= -1) {
-                t = rs.rates[rs.file_rate[r.file]];
-                N = cc.file_len[r.file];
-                const int64_t Nt = t.taps ? (int64_t)(((uint64_t)N * t.n + t.o - 1) / t.o) : N;  // (N < 2^36, n < 2^20)
-                if (r.offset <= Nt) {
-                    const int64_t rest = Nt - r.offset;
-                    len = r.length == -1 || r.length > rest ? rest : r.length;
-                    valid = true;
-                }
-            }
-        }
-        const uint64_t cols = ((uint64_t)len + 3) & ~(uint64_t)3;
-        const uint64_t start = cta_scan(PackedSums{cols, 0, 0, 0}, s_warp, &s_cols).cols;
-        const bool fit = valid && start + (uint64_t)len <= pb.T;
-        clx_packed_request q{0, 1, 0, 1};  // invalid (reserved != 0): status CLX_ERR_INVALID_ARGUMENT, nothing decoded
-        ResamplePlan p{0, 0, 0, 0, 0};
-        if (fit) {
-            int64_t lo, hi;
-            source_span(t, N, r.offset, len, &lo, &hi);
-            q = clx_packed_request{r.file, 0, lo, len > 0 ? hi - lo : -1};
-            p = ResamplePlan{r.offset, lo, hi - lo, rs.file_rate[r.file], cc.file_ch[r.file]};
-        }
-        if (i < n) {
-            pb.starts[i] = (int64_t)start;
-            rs.lengths[i] = fit ? len : 0;
-            rs.plan[i] = p;
-            rs.excerpts[i] = q;
-        }
-    }
-}
+// output's row stride; eb holds the caller's requests and count at rate R, and the target column starts.
 
 // Grid: x over tiles of rs.tile columns, y over the rows.  The CTA of columns [c0, c0 + tile) walks the excerpts that
 // overlap them, from the first one that ends after c0 (found by binary search: the ends start_b + n_b never decrease,
@@ -234,21 +208,21 @@ resample_packed_map_kernel(CropCorpus cc, ResampleBuffers rs, PackedBuffers pb) 
 // body, or a copy at r == R; every other column of the range is written 0, so nothing is left from an earlier call.
 // A tile of many short excerpts runs the body once per excerpt, each with its own staging and two barriers.
 __global__ void __launch_bounds__(RS_THREADS)
-resample_packed_kernel(ResampleBuffers rs, PackedBuffers pb) {
+resample_packed_kernel(ResampleBuffers rs, ExcerptBuffers eb) {
     __shared__ float s_x[RS_SMEM];
     const uint32_t c = blockIdx.y;
     const uint64_t c0 = (uint64_t)blockIdx.x * rs.tile, ce = min(c0 + rs.tile, rs.L);
     float* out = rs.out + (uint64_t)c * rs.L;
-    const uint32_t used = min(*pb.count, rs.n_crops);
+    const uint32_t used = min(*eb.count, rs.n_crops);
     uint32_t b = 0, e = used;
     while (b < e) {
         const uint32_t mid = (b + e) >> 1;
-        if ((uint64_t)(pb.starts[mid] + rs.lengths[mid]) > c0) e = mid;
+        if ((uint64_t)(eb.starts[mid] + rs.lengths[mid]) > c0) e = mid;
         else b = mid + 1;
     }
     uint64_t z = c0;  // columns [c0, z) are written
     for (; b < used; b++) {
-        const uint64_t start = (uint64_t)pb.starts[b], len = (uint64_t)rs.lengths[b];
+        const uint64_t start = (uint64_t)eb.starts[b], len = (uint64_t)rs.lengths[b];
         if (start >= ce) break;
         if (len == 0) continue;
         const uint64_t lo = max(start, c0), hi = min(start + len, ce);
@@ -273,17 +247,10 @@ resample_packed_kernel(ResampleBuffers rs, PackedBuffers pb) {
     for (uint64_t j = z + threadIdx.x; j < ce; j += RS_THREADS) out[j] = 0.f;
 }
 
-cudaError_t launch_resample_packed_map(const CropCorpus& cc, const ResampleBuffers& rs, const PackedBuffers& pb,
-                                       cudaStream_t stream, uint64_t* launches) {
-    resample_packed_map_kernel<<<1, SCAN_THREADS, 0, stream>>>(cc, rs, pb);
-    (*launches)++;
-    return cudaGetLastError();
-}
-
-cudaError_t launch_resample_packed(const ResampleBuffers& rs, const PackedBuffers& pb, cudaStream_t stream,
+cudaError_t launch_resample_packed(const ResampleBuffers& rs, const ExcerptBuffers& eb, cudaStream_t stream,
                                    uint64_t* launches) {
     const dim3 grid((uint32_t)((rs.L + rs.tile - 1) / rs.tile), rs.C);
-    resample_packed_kernel<<<grid, RS_THREADS, 0, stream>>>(rs, pb);
+    resample_packed_kernel<<<grid, RS_THREADS, 0, stream>>>(rs, eb);
     (*launches)++;
     return cudaGetLastError();
 }

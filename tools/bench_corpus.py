@@ -55,22 +55,23 @@ def gathered_bytes(corpus, fi, off, n):
     return total
 
 
-def profile_kernels(batch, draws):
-    """Device time per call of each crop_* kernel (us), from a torch.profiler run of its own."""
+def profile_kernels(call, items, match):
+    """Device time per call(x), x in items, of each kernel whose name contains `match` (us), from a torch.profiler run
+    of its own.  Kernels are named without namespace and template arguments: "void clx::k<clx::CropLayout>(...)" is k."""
     import torch
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for fi, off in draws:
-            batch(fi, off, check=False)
+        for x in items:
+            call(x)
         torch.cuda.synchronize()
     us = {}
     for e in prof.key_averages():
         t = getattr(e, "device_time_total", None)
         t = getattr(e, "cuda_time_total", 0) if t is None else t
-        if t and "crop_" in e.key:
-            name = e.key.split("(")[0].split("::")[-1].split("<")[0].strip()
-            us[name] = round(us.get(name, 0.0) + t / len(draws), 2)
+        if t and match in e.key:
+            name = e.key.split("(")[0].split("<")[0].split("::")[-1].split()[-1]
+            us[name] = round(us.get(name, 0.0) + t / len(items), 2)
     return us
 
 
@@ -172,9 +173,9 @@ def main():
     info = gpu_info()
     for dev in win:
         dev.close()
-    kernels_us = profile_kernels(hbatch, draws[:args.profile_calls])
+    kernels_us = profile_kernels(lambda d: hbatch(*d, check=False), draws[:args.profile_calls], "excerpt_")
     prof_bytes = float(np.mean(per_call[:args.profile_calls]))
-    gather_us = kernels_us.get("crop_gather_kernel")
+    gather_us = kernels_us.get("excerpt_gather_kernel")
     host_ms = float(np.median(ms["host_corpus_crop_batch_device"]))
     gathered.update({"gather_kernel_GBps": round(prof_bytes / (gather_us * 1e3), 2) if gather_us else None,
                      "over_whole_call_GBps": round(gathered["mean_per_call"] / (host_ms * 1e6), 2)})

@@ -11,7 +11,7 @@ Every draw is checked bit for bit against load() of the same files once.  Then, 
 4. a CropBatch with L = the longest file of any draw, B = the most files of a draw and offsets 0 (files past a draw's
    end get offset = length, so no frames): the padded layout, device time per call.
 
-A torch.profiler run gives each packed_* kernel's own time per call (the planner's cost).  Memory of each (output,
+A torch.profiler run gives each excerpt_* kernel's own time per call (the planner's cost).  Memory of each (output,
 planar scratch, staging) and the byte bound against the bytes actually gathered are reported, with the card's name,
 power limit and SM clock read in the same run.  One JSON line.
 
@@ -32,7 +32,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 import claxon_b200 as cb  # noqa: E402
 from claxon_b200 import synth  # noqa: E402
-from tools.bench_corpus import stats  # noqa: E402
+from tools.bench_corpus import profile_kernels, stats  # noqa: E402
 from tools.bench_out_modes import gpu_info  # noqa: E402
 
 
@@ -61,24 +61,6 @@ def draw(idx, T, rng):
 def span_bytes(corpus, files):
     return sum(int(corpus.index[f].descs["byte_offset"][-1]) + int(corpus.index[f].descs["byte_len"][-1])
                - int(corpus.index[f].descs["byte_offset"][0]) for f in files)
-
-
-def profile_kernels(batch, draws):
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for files in draws:
-            batch(files, check=False)
-        torch.cuda.synchronize()
-    us = {}
-    for e in prof.key_averages():
-        t = getattr(e, "device_time_total", None)
-        t = getattr(e, "cuda_time_total", 0) if t is None else t
-        if t and "packed_" in e.key:
-            name = e.key.split("(")[0].split("::")[-1].split("<")[0].strip()
-            us[name] = round(us.get(name, 0.0) + t / len(draws), 2)
-    return us
 
 
 def main():
@@ -159,7 +141,8 @@ def main():
         ms["load_host"].append(float(np.median(per)))
         ms["crop_batch_padded_device"].append(device_ms(lambda c: crops(*c, check=False), crop_draws))
     info = gpu_info()
-    kernels_us = {"device": profile_kernels(packed, draws[:10]), "host_corpus": profile_kernels(hpacked, draws[:10])}
+    kernels_us = {"device": profile_kernels(lambda d: packed(d, check=False), draws[:10], "excerpt_"),
+                  "host_corpus": profile_kernels(lambda d: hpacked(d, check=False), draws[:10], "excerpt_")}
     samples = float(np.mean([sum(idx[f].length for f in d) for d in draws]))
     row = {"bench": "packed", "T": T, "draws": args.draws, "rounds": args.rounds, "files_per_draw_mean": float(np.mean([len(d) for d in draws])),
            "samples_per_draw_mean": samples, "bit_exact_vs_load_and_host_corpus": exact,

@@ -29,7 +29,7 @@ sys.path.insert(0, ROOT)
 import claxon_b200 as cb  # noqa: E402
 from claxon_b200 import synth  # noqa: E402
 from tests import spec_resample as S  # noqa: E402
-from tools.bench_corpus import stats  # noqa: E402
+from tools.bench_corpus import profile_kernels, stats  # noqa: E402
 from tools.bench_out_modes import gpu_info  # noqa: E402
 
 
@@ -59,24 +59,6 @@ def created(make):
     batch = make()
     torch.cuda.synchronize()
     return batch, free0 - torch.cuda.mem_get_info()[0]
-
-
-def profile_kernels(call, items, match):
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for x in items:
-            call(x)
-        torch.cuda.synchronize()
-    us = {}
-    for e in prof.key_averages():
-        t = getattr(e, "device_time_total", None)
-        t = getattr(e, "cuda_time_total", 0) if t is None else t
-        if t and match in e.key:
-            name = e.key.split("(")[0].split("::")[-1].split("<")[0].strip()
-            us[name] = round(us.get(name, 0.0) + t / len(items), 2)
-    return us
 
 
 def main():

@@ -134,14 +134,12 @@ def main():
             for name, call in calls.items():
                 ms[name].append(device_ms(call, items[name.split("_")[0]]))
         info = gpu_info()
-        kernels_us = {"crops_host": bench_corpus.profile_kernels(hb, draws[:args.profile_calls]),
-                      "crops_attached": bench_corpus.profile_kernels(ab, draws[:args.profile_calls]),
-                      "packed_host": bench_packed.profile_kernels(hp, pdraws[:args.profile_calls]),
-                      "packed_attached": bench_packed.profile_kernels(ap_, pdraws[:args.profile_calls])}
+        kernels_us = {name: bench_corpus.profile_kernels(call, items[name.split("_")[0]][:args.profile_calls],
+                                                         "excerpt_") for name, call in calls.items()}
         gbps = {}
         for name in calls:
             nbytes = crop_bytes if name.startswith("crops") else packed_bytes
-            gather = kernels_us[name].get("crop_gather_kernel" if name.startswith("crops") else "packed_gather_kernel")
+            gather = kernels_us[name].get("excerpt_gather_kernel")
             gbps[name] = {"over_call": round(nbytes / (float(np.median(ms[name])) * 1e6), 2),
                           "over_gather_kernel": round(nbytes / (gather * 1e3), 2) if gather else None}
         del hb, ab, hp, ap_

@@ -24,7 +24,8 @@ from ._lib import (OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT)
 from ._lib import (FrameDesc, FrameResult, FrameWindow, OPT_NO_VERIFY_CRC, OPT_GENERIC_KERNEL_ONLY, OPT_WARP_PER_FRAME, OPT_LANE_PER_FRAME,
                    OPT_NO_GENERIC, OPT_NO_WIDE, FRAME_VARIABLE_BLOCKING, FRAME_CRC16_VERIFIED,
                    OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24,
-                   OUT_CHANNELS_I32, OUT_CHANNELS_F32, MEL_CENTER, MEL_LOG)
+                   OUT_CHANNELS_I32, OUT_CHANNELS_F32, MEL_CENTER, MEL_LOG, MEL_NORM_PER_FEATURE,
+                   MEL_NORM_WHISPER)
 
 __all__ = ["Error", "Block", "FrameReader", "FlacReader", "FlacReaderOptions", "StreamInfo", "Context", "DeviceBatch",
            "parse_frame_header", "demux_frames", "open_stream", "ogg_frames", "mp4_frames", "status_str", "DESC_DTYPE", "RESULT_DTYPE", "load", "plan_columns",
@@ -1034,14 +1035,15 @@ class Corpus:
                   win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
                   f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
                   center: bool = True, norm: str | None = None, mel_scale: str = "htk",
-                  log_floor: float | None = None) -> "MelCropBatch":
+                  log_floor: float | None = None, normalize: str | None = None) -> "MelCropBatch":
         """A MelCropBatch: the mel spectrogram of each crop of a crop batch of `batch` crops of `num_frames` samples
         (resampled to `sample_rate` when given), computed on the device.  The keywords are those of
         torchaudio.transforms.MelSpectrogram (window_fn None is torch.hann_window); log_floor None gives the power,
-        a float ln(max(mel, log_floor))."""
+        a float ln(max(mel, log_floor)); normalize None, "per_feature" or "whisper" (see MelCropBatch)."""
         return MelCropBatch(self, batch, num_frames, sample_rate, n_fft=n_fft, win_length=win_length,
                             hop_length=hop_length, f_min=f_min, f_max=f_max, n_mels=n_mels, window_fn=window_fn,
-                            wkwargs=wkwargs, center=center, norm=norm, mel_scale=mel_scale, log_floor=log_floor)
+                            wkwargs=wkwargs, center=center, norm=norm, mel_scale=mel_scale, log_floor=log_floor,
+                            normalize=normalize)
 
     def resample_source_bound(self, num_frames: int, sample_rate: int) -> int:
         """The most source samples a crop of num_frames samples at `sample_rate` reads from one file of the corpus
@@ -1070,13 +1072,14 @@ class Corpus:
                    win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
                    f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
                    center: bool = True, norm: str | None = None, mel_scale: str = "htk",
-                   log_floor: float | None = None) -> "MelPackedBatch":
+                   log_floor: float | None = None, normalize: str | None = None) -> "MelPackedBatch":
         """A MelPackedBatch: the mel spectrogram of each excerpt of a packed batch of up to `max_excerpts` excerpts
         along `max_samples` columns (resampled to `sample_rate` when given), packed along frames, computed on the
-        device.  The keywords are mel_crops()'s."""
+        device.  The keywords are mel_crops()'s, but normalize is None or "per_feature"."""
         return MelPackedBatch(self, max_excerpts, max_samples, sample_rate, n_fft=n_fft, win_length=win_length,
                               hop_length=hop_length, f_min=f_min, f_max=f_max, n_mels=n_mels, window_fn=window_fn,
-                              wkwargs=wkwargs, center=center, norm=norm, mel_scale=mel_scale, log_floor=log_floor)
+                              wkwargs=wkwargs, center=center, norm=norm, mel_scale=mel_scale, log_floor=log_floor,
+                              normalize=normalize)
 
     def mel_packed_frames_bound(self, max_excerpts: int, max_samples: int, *, n_fft: int = 400,
                                 win_length: int | None = None, hop_length: int | None = None,
@@ -1434,11 +1437,19 @@ def _mel_rate(index: FlacIndex, sample_rate: int | None) -> int:
     return rates.pop()
 
 
+_MEL_NORMALIZE = {None: 0, "per_feature": MEL_NORM_PER_FEATURE, "whisper": MEL_NORM_WHISPER}
+
+
 def _mel_tables(sample_rate: int, n_fft: int, win_length, hop_length, f_min: float, f_max, n_mels: int, window_fn,
-                wkwargs, center: bool, norm, mel_scale: str, log_floor):
-    """MelSpectrogram's arguments as (clx_mel_params, window [win_length] float32, fbank [n_fft // 2 + 1, n_mels]
-    float32); the C ABI checks the ranges."""
+                wkwargs, center: bool, norm, mel_scale: str, log_floor, normalize=None):
+    """MelSpectrogram's arguments and `normalize` as (clx_mel_params, window [win_length] float32, fbank [n_fft // 2 +
+    1, n_mels] float32); the C ABI checks the ranges."""
     import torch
+    if normalize not in _MEL_NORMALIZE:
+        raise ValueError('normalize must be None, "per_feature" or "whisper"')
+    if normalize is not None and (log_floor is None or not center):
+        raise ValueError(f'normalize="{normalize}" works on log features of centred frames: it needs log_floor and '
+                         'center=True')
     n_fft, n_mels = int(n_fft), int(n_mels)
     win_length = n_fft if win_length is None else int(win_length)
     hop_length = win_length // 2 if hop_length is None else int(hop_length)
@@ -1457,7 +1468,8 @@ def _mel_tables(sample_rate: int, n_fft: int, win_length, hop_length, f_min: flo
         raise ValueError(f"window_fn gave {window.size} values for win_length {win_length}")
     fbank = np.ascontiguousarray(melscale_fbanks(n_fft // 2 + 1, f_min, f_max, n_mels, sample_rate, norm, mel_scale),
                                  dtype=np.float32)
-    params = _lib.MelParams(n_fft, win_length, hop_length, n_mels, flags, 0.0 if log_floor is None else log_floor)
+    params = _lib.MelParams(n_fft, win_length, hop_length, n_mels, flags | _MEL_NORMALIZE[normalize],
+                            0.0 if log_floor is None else log_floor)
     return params, window, fbank
 
 
@@ -1474,16 +1486,30 @@ class MelCropBatch(CropBatch):
     (ln(log_floor) with the log); a failed crop's are unspecified.  lengths and status are the crop batch's, lengths in
     samples at the crop's rate.  The filterbank's rate is `sample_rate`, else the corpus's single rate (ValueError for
     a corpus of mixed rates).  n_fft must be even, 8 to 4096, with n_fft / 2 a product of 2, 3 and 5; n_mels at most
-    512; L above n_fft / 2 with center, at least n_fft without (Error 90 otherwise)."""
+    512; L above n_fft / 2 with center, at least n_fft without (Error 90 otherwise).
+
+    `normalize` (log_floor and center required, else ValueError) normalises the log features on the device, in the
+    same graph, each statistic and map in float64 rounded once to float32; calls stay bit-identical.
+    * "per_feature": for each (crop b, row, mel), over its first v_b = 1 + n_b // hop_length frames (n_b = lengths[b];
+      v_b = 0 when n_b = 0), y = (x - mean) / (std + 1e-5) with the unbiased std (0 for one frame): NeMo's per_feature
+      normalize_batch, with torch.stft's frame count of the crop's valid samples.  Frames from v_b on read exactly 0,
+      and so does every frame of an invalid crop and of a row the file lacks.
+    * "whisper": transformers.WhisperFeatureExtractor's log-mel of each crop row as its (zero-padded) input: F - 1
+      frames (n_frames; Whisper drops the last STFT frame), l = x / ln 10 and y = (max(l, M - 8) + 4) / 4 with M the
+      row's largest l.  Whisper's own features come from mel_crops(B, 480000, 16000, n_fft=400, hop_length=160,
+      n_mels=80 (or 128 for large-v3), mel_scale="slaney", norm="slaney", log_floor=1e-10, normalize="whisper"): 30 s
+      at 16 kHz, 3000 frames."""
 
     def __init__(self, corpus: Corpus, batch: int, num_frames: int, sample_rate: int | None = None, *,
                  n_fft: int = 400, win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
                  f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
-                 center: bool = True, norm: str | None = None, mel_scale: str = "htk", log_floor: float | None = None):
+                 center: bool = True, norm: str | None = None, mel_scale: str = "htk", log_floor: float | None = None,
+                 normalize: str | None = None):
         self._args(corpus, batch, num_frames, None, sample_rate)
         params, window, fbank = _mel_tables(_mel_rate(corpus.index, self.sample_rate), n_fft, win_length, hop_length,
                                             f_min, f_max, n_mels, window_fn, wkwargs, center, norm, mel_scale,
-                                            log_floor)
+                                            log_floor, normalize)
+        self.normalize = normalize
         self.params, self.fbank, self.window = params, fbank, window
         L = self.ctx._L
         h = C.c_void_p()
@@ -1492,7 +1518,7 @@ class MelCropBatch(CropBatch):
                                             window.ctypes.data, fbank.ctypes.data, C.byref(h)), self.ctx)
         self.channels, self.n_mels = corpus.channels, params.n_mels
         self.n_frames = (1 + self.num_frames // params.hop_length if center else
-                         1 + (self.num_frames - params.n_fft) // params.hop_length)
+                         1 + (self.num_frames - params.n_fft) // params.hop_length) - (normalize == "whisper")
         self._attach(h, (self.batch, self.channels, self.n_mels, self.n_frames), "<f4")
 
 
@@ -1671,16 +1697,25 @@ class MelPackedBatch(PackedBatch):
     round_up_4(frames[b]); every other element of the features reads exactly 0 after every call, with or without the
     log.  T_f = Corpus.mel_packed_frames_bound(max_excerpts, max_samples, ...) holds the frames of any excerpts that fit
     in max_samples columns, so only the packed batch's fit rule applies.  Calls are bit-identical.  Memory: the packed
-    batch and C x n_mels x T_f float32."""
+    batch and C x n_mels x T_f float32.
+
+    normalize="per_feature" (log_floor and center required) normalises each (excerpt b, row, mel) over its F_b frames
+    as MelCropBatch does a crop's valid frames: y = (x - mean) / (std + 1e-5), unbiased std, 0 for one frame; the
+    layout, starts and frame counts are unchanged and every other element still reads 0.  "whisper" is refused
+    (ValueError): Whisper's input is a fixed 30 s window, and per-excerpt maxima match no reference."""
 
     def __init__(self, corpus: Corpus, max_excerpts: int, max_samples: int, sample_rate: int | None = None, *,
                  n_fft: int = 400, win_length: int | None = None, hop_length: int | None = None, f_min: float = 0.0,
                  f_max: float | None = None, n_mels: int = 128, window_fn=None, wkwargs: dict | None = None,
-                 center: bool = True, norm: str | None = None, mel_scale: str = "htk", log_floor: float | None = None):
+                 center: bool = True, norm: str | None = None, mel_scale: str = "htk", log_floor: float | None = None,
+                 normalize: str | None = None):
+        if normalize == "whisper":
+            raise ValueError('normalize="whisper" is for crop batches (Whisper reads fixed 30 s windows)')
         self._args(corpus, max_excerpts, max_samples, None, sample_rate)
         params, window, fbank = _mel_tables(_mel_rate(corpus.index, self.sample_rate), n_fft, win_length, hop_length,
                                             f_min, f_max, n_mels, window_fn, wkwargs, center, norm, mel_scale,
-                                            log_floor)
+                                            log_floor, normalize)
+        self.normalize = normalize
         self.params, self.fbank, self.window = params, fbank, window
         L = self.ctx._L
         h = C.c_void_p()

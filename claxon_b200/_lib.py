@@ -74,6 +74,7 @@ OPEN_METADATA_ONLY, OPEN_NO_VORBIS_COMMENT = 1, 2
 BATCH_BYTES_ON_DEVICE = 1
 CORPUS_HOST = 1
 MEL_CENTER, MEL_LOG = 1, 2
+MEL_NORM_PER_FEATURE, MEL_NORM_WHISPER = 4, 8
 IMAGE_MAGIC, IMAGE_VERSION, IMAGE_ALIGN, IMAGE_END_CONFIRMED = 0x3150524F43584C43, 1, 4096, 1
 OUT_PLANAR_I32, OUT_INTERLEAVED_I32, OUT_INTERLEAVED_I16, OUT_INTERLEAVED_I24 = 0, 1, 2, 3
 OUT_CHANNELS_I32, OUT_CHANNELS_F32 = 4, 5

@@ -243,6 +243,7 @@ struct clx_batch {
     clx::MelBuffers mel{};
     size_t mel_smem = 0;
     clx::MelPacked mel_packed{};
+    clx::MelNorm mel_norm{};  // flags 0 without a CLX_MEL_NORM_* flag
 };
 
 struct clx_corpus {
@@ -701,10 +702,11 @@ cudaError_t launch_batch(clx_batch* b, cudaStream_t st, uint64_t* launches) {
         return e == cudaSuccess ? clx::launch_resample_packed(b->rs, b->ex, st, launches) : e;
     case Kind::MelCrops:
         e = launch_batch(b->inner, st, launches);
-        return e == cudaSuccess ? clx::launch_mel(b->mel, b->mel_smem, st, launches) : e;
+        return e == cudaSuccess ? clx::launch_mel(b->mel, b->mel_norm, b->mel_smem, st, launches) : e;
     case Kind::MelPacked:
         e = launch_batch(b->inner, st, launches);
-        return e == cudaSuccess ? clx::launch_mel_packed(b->mel, b->mel_packed, b->mel_smem, st, launches) : e;
+        return e == cudaSuccess ? clx::launch_mel_packed(b->mel, b->mel_packed, b->mel_norm, b->mel_smem, st, launches)
+                                : e;
     }
     return cudaErrorInvalidValue;
 }
@@ -1403,6 +1405,13 @@ cudaError_t fill_mel(clx_batch* b, const clx_mel_params* p, const clx::MelTables
     if (e == cudaSuccess) e = upload(b, mb.bands, t.bands);
     if (e == cudaSuccess) e = upload(b, mb.weights, t.weights);
     mb.out = reinterpret_cast<float*>(b->buf.conv);
+    clx::MelNorm& mn = b->mel_norm;  // the layout fields; the caller sets the lengths or the packed plan
+    mn.out = mb.out;
+    mn.F = F;
+    mn.C = b->corpus->channels;
+    mn.n_mels = p->n_mels;
+    mn.hop = p->hop_length;
+    mn.flags = p->flags & (CLX_MEL_NORM_PER_FEATURE | CLX_MEL_NORM_WHISPER);
     return e;
 }
 
@@ -1412,11 +1421,15 @@ int make_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates,
     if (!ctx || !corpus || n_crops == 0 || n_crops >= (1u << 30)) return CLX_ERR_INVALID_ARGUMENT;
     clx::MelTables t;
     if (!clx::mel_tables(params, window, fbank, &t)) return CLX_ERR_INVALID_ARGUMENT;
-    const uint64_t F = clx::mel_frame_count(num_frames, params->n_fft, params->hop_length, params->flags & CLX_MEL_CENTER);
+    const bool whisper = params->flags & CLX_MEL_NORM_WHISPER;
+    uint64_t F = clx::mel_frame_count(num_frames, params->n_fft, params->hop_length, params->flags & CLX_MEL_CENTER);
     if (F == 0) return CLX_ERR_INVALID_ARGUMENT;  // a row too short for a frame, or for the reflect pad
+    if (whisper && F-- < 2) return CLX_ERR_INVALID_ARGUMENT;  // Whisper drops the last frame: it needs two
     const size_t C = corpus->channels, rows = n_crops * C;  // (< 2^33: no overflow)
     const uint64_t tiles = (F + t.tile - 1) / t.tile;
     if (F > (SIZE_MAX / 4 - 8) / (rows * params->n_mels) || tiles >= (1u << 31) / rows) return CLX_ERR_INVALID_ARGUMENT;
+    if ((params->flags & CLX_MEL_NORM_PER_FEATURE) && rows * params->n_mels >= (1u << 31))
+        return CLX_ERR_INVALID_ARGUMENT;  // mel_norm_kernel numbers its (row, mel) segments in 32 bits
     clx_batch* inner = nullptr;
     const int rc = target_rate ? make_resampled_crops(ctx, corpus, file_rates, n_files, n_crops, num_frames,
                                                       target_rate, &inner, e)
@@ -1424,6 +1437,8 @@ int make_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates,
     if (rc != CLX_OK) return rc;
     clx_batch* b = *out = new_batch(Kind::MelCrops, corpus, inner);
     if (*e == cudaSuccess) *e = fill_mel(b, params, t, F, rows, tiles);
+    b->mel_norm.lengths = b->ex.lengths;
+    b->mel_norm.n = (uint32_t)n_crops;
     return CLX_OK;
 }
 
@@ -1433,11 +1448,14 @@ int make_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates
     if (!ctx || !corpus || max_excerpts == 0 || max_excerpts >= (1u << 30) || max_samples == 0)
         return CLX_ERR_INVALID_ARGUMENT;
     clx::MelTables t;
-    if (!clx::mel_tables(params, window, fbank, &t)) return CLX_ERR_INVALID_ARGUMENT;
+    if (!clx::mel_tables(params, window, fbank, &t) || (params->flags & CLX_MEL_NORM_WHISPER))
+        return CLX_ERR_INVALID_ARGUMENT;  // (Whisper's input is a fixed window: crops only)
     const size_t F = clx::mel_packed_frames(params, max_excerpts, max_samples), C = corpus->channels;
     const uint64_t tiles = std::max<uint64_t>(1, (F + t.tile - 1) / t.tile);  // (one CTA per row when F is 0)
     if (F == SIZE_MAX || F > (SIZE_MAX / 4 - 8) / (C * params->n_mels) || tiles >= (1u << 31) / C)
         return CLX_ERR_INVALID_ARGUMENT;
+    if ((params->flags & CLX_MEL_NORM_PER_FEATURE) && max_excerpts * C * params->n_mels >= (1u << 31))
+        return CLX_ERR_INVALID_ARGUMENT;  // mel_norm_kernel numbers its (excerpt, row, mel) segments in 32 bits
     clx_batch* inner = nullptr;
     const int rc = target_rate ? make_resampled_packed(ctx, corpus, file_rates, n_files, max_excerpts, max_samples,
                                                        target_rate, &inner, e)
@@ -1453,6 +1471,10 @@ int make_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates
     if (*e == cudaSuccess) *e = device_zeros(b, b->ex.starts, max_excerpts);
     if (*e == cudaSuccess) *e = device_zeros(b, mp.frames, max_excerpts);
     mp.starts = b->ex.starts;
+    b->mel_norm.count = mp.count;
+    b->mel_norm.starts = mp.starts;
+    b->mel_norm.frames = mp.frames;
+    b->mel_norm.n = mp.n;
     return CLX_OK;
 }
 

@@ -228,7 +228,8 @@ size_t resample_packed_bound(const ResampleTables& t, size_t max_excerpts, size_
 cudaError_t launch_resample_packed(const ResampleBuffers& rs, const ExcerptBuffers& eb, cudaStream_t stream,
                                    uint64_t* launches);
 
-// clx_mel.cu: mel crop batches (clx_batch_create_mel_crops), one kernel after an inner crop or resampled crop batch.
+// clx_mel.cu: mel crop batches (clx_batch_create_mel_crops), one kernel after an inner crop or resampled crop batch
+// (two with a CLX_MEL_NORM_* flag).
 // Mel m sums weights[w + i] * |X[lo + i]|^2 for i < n: the non-zero span of its filterbank column.
 struct MelBand {
     uint32_t lo, n, w;
@@ -258,7 +259,20 @@ struct MelTables {
 bool mel_params_ok(const clx_mel_params* p);
 bool mel_tables(const clx_mel_params* p, const float* window, const float* fbank, MelTables* t);
 cudaError_t mel_init();  // the mel kernels' shared memory limit, on the current device, before a graph captures them
-cudaError_t launch_mel(const MelBuffers& mb, size_t smem, cudaStream_t stream, uint64_t* launches);
+// mel_norm_kernel's view of a mel batch with CLX_MEL_NORM_* in flags (flags 0: no normalisation, no launch).  Crops:
+// segment (crop b, row c, mel m) is out[((b C + c) n_mels + m) F ...], its valid frames 1 + lengths[b] / hop.  Packed
+// (count set): out[(c n_mels + m) F + starts[b] ...], frames[b] of them, for b < min(*count, n).
+struct MelNorm {
+    float* out;
+    const int64_t* lengths;  // crops: each crop's length in samples
+    const uint32_t* count;   // packed: the call's excerpt count; NULL for crops
+    const int64_t* starts;   // packed: frame starts and counts (the planner's)
+    const int64_t* frames;
+    uint64_t F;              // the row pitch: frames of a crop row, T_f of a packed batch
+    uint32_t n, C, n_mels, hop;  // n: crops, or max_excerpts
+    uint32_t flags;          // CLX_MEL_NORM_PER_FEATURE or CLX_MEL_NORM_WHISPER, or 0
+};
+cudaError_t launch_mel(const MelBuffers& mb, const MelNorm& mn, size_t smem, cudaStream_t stream, uint64_t* launches);
 // Mel packed batches (clx_batch_create_mel_packed) keep a MelBuffers with src = the inner packed batch's [C, L] output
 // (L its row stride), rows = C, F = the frame columns T_f (the features' row pitch), and this: the inner batch's count,
 // lengths in samples and sample starts, and the batch's own frame starts and frame counts, written by the planner.
@@ -272,9 +286,10 @@ struct MelPacked {
 };
 // clx_mel_packed_frames_bound of valid parameters: SIZE_MAX if it overflows.
 size_t mel_packed_frames(const clx_mel_params* p, size_t max_excerpts, size_t max_samples);
-// The planner (frame counts and starts) and mel_packed_kernel, after the inner batch's launch sequence.
-cudaError_t launch_mel_packed(const MelBuffers& mb, const MelPacked& mp, size_t smem, cudaStream_t stream,
-                              uint64_t* launches);
+// The planner (frame counts and starts), mel_packed_kernel and, with mn.flags, mel_norm_kernel, after the inner batch's
+// launch sequence.
+cudaError_t launch_mel_packed(const MelBuffers& mb, const MelPacked& mp, const MelNorm& mn, size_t smem,
+                              cudaStream_t stream, uint64_t* launches);
 #ifdef CLX_EXPERIMENT
 extern int g_exp_which;  // measurement builds only: bit 0 = index pass, bit 1 = decode pass of LanePerFrame
 extern int g_exp_dyn_smem;

@@ -12,6 +12,10 @@
 // mel_packed_plan_kernel gives each excerpt its frame count and frame start, and mel_packed_kernel computes the frames
 // of one (tile of frame columns, row) per CTA with mel_kernel's per-frame arithmetic, once over the whole tile whatever
 // the excerpts in it.
+//
+// With CLX_MEL_NORM_PER_FEATURE or CLX_MEL_NORM_WHISPER, mel_norm_kernel follows either mel kernel and normalises the
+// log features in place: per (crop or excerpt, row, mel) mean and variance over the valid frames, or Whisper's clamp
+// and rescale per crop row.  The mel kernels do not change; for Whisper, mel_kernel just runs with F - 1 frames.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -249,6 +253,98 @@ mel_packed_kernel(MelBuffers mb, MelPacked mp) {
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// mel_norm_kernel: the CLX_MEL_NORM_* maps, in place over the log features the mel kernel wrote.  Statistics and maps
+// are float64, rounded once to float32; every reduction has one fixed order and no atomics, so calls are bit-identical
+// and a constant segment gives exactly 0 (its partial sums k x are exact in float64, so mu = x).
+
+constexpr uint32_t MEL_NORM_THREADS = 512;
+constexpr uint32_t MEL_NORM_MAX_CTAS = 1u << 20;  // per-feature CTAs loop over the segments past that
+constexpr double MEL_LOG10_E = 0.434294481903251827651;  // 1 / ln 10
+
+// The sum of v over a warp, by xor butterflies: every lane adds the same two values at each step, so all lanes get
+// the same sum.
+__device__ __forceinline__ double mel_warp_sum(double v) {
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// CLX_MEL_NORM_PER_FEATURE: one warp per segment (crop or excerpt b, row c, mel m), segments numbered b-major.  Three
+// walks over the segment's contiguous frames, lane t mod 32 taking frame t: the sum, the squared deviations from the
+// mean, then the map in place (a crop's frames past v written 0).  The last two walks read what the first brought
+// into L1 / L2.
+__device__ __forceinline__ void mel_norm_per_feature(const MelNorm& mn) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t segs = mn.n * mn.C * mn.n_mels, warps = gridDim.x * (MEL_NORM_THREADS / 32);  // (< 2^31: create)
+    const uint32_t used = mn.count ? min(*mn.count, mn.n) : mn.n;
+    for (uint32_t s = (blockIdx.x * MEL_NORM_THREADS + threadIdx.x) / 32; s < segs; s += warps) {
+        const uint32_t rc = s / mn.n_mels;  // b C + c
+        const uint32_t m = s - rc * mn.n_mels, b = rc / mn.C, c = rc - b * mn.C;
+        if (b >= used) break;  // (s only grows)
+        float* x;
+        uint64_t v, F;
+        if (mn.count) {  // packed: F_b frames at start_b, nothing else to write
+            v = F = (uint64_t)mn.frames[b];
+            x = mn.out + ((uint64_t)c * mn.n_mels + m) * mn.F + mn.starts[b];
+        } else {  // crops: torch.stft's frame count of the crop's n_b samples, 0 for none
+            const int64_t n = mn.lengths[b];
+            v = n > 0 ? min(mn.F, 1 + (uint64_t)n / mn.hop) : 0;
+            F = mn.F;
+            x = mn.out + (uint64_t)s * mn.F;
+        }
+        double sum = 0.0;
+        for (uint64_t t = lane; t < v; t += 32) sum += (double)x[t];
+        const double mu = mel_warp_sum(sum) / (double)v;
+        double dev = 0.0;
+        for (uint64_t t = lane; t < v; t += 32) {
+            const double d = (double)x[t] - mu;
+            dev = fma(d, d, dev);
+        }
+        const double sigma = v > 1 ? sqrt(mel_warp_sum(dev) / (double)(v - 1)) : 0.0, den = sigma + 1e-5;
+        for (uint64_t t = lane; t < F; t += 32) x[t] = t < v ? (float)(((double)x[t] - mu) / den) : 0.f;
+    }
+}
+
+// CLX_MEL_NORM_WHISPER: one CTA per row of [n_mels, F'] features.  The row's largest x (the largest l as well: the
+// scaling keeps the order), then y = (max(l, M - 8) + 4) / 4 in place, l = x log10(e) (within an ulp of x / ln 10 in
+// float64, far below the float32 rounding).
+__device__ __forceinline__ void mel_norm_whisper(const MelNorm& mn) {
+    __shared__ float s_max[MEL_NORM_THREADS / 32];
+    const uint64_t n = (uint64_t)mn.n_mels * mn.F;
+    float* x = mn.out + (uint64_t)blockIdx.x * n;
+    float hi = -INFINITY;
+#pragma unroll 4
+    for (uint64_t i = threadIdx.x; i < n; i += MEL_NORM_THREADS) hi = fmaxf(hi, x[i]);
+    for (int o = 16; o; o >>= 1) hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x / 32] = hi;
+    __syncthreads();
+    hi = s_max[0];
+    for (uint32_t w = 1; w < MEL_NORM_THREADS / 32; w++) hi = fmaxf(hi, s_max[w]);
+    const double lo = (double)hi * MEL_LOG10_E - 8.0;
+#pragma unroll 4
+    for (uint64_t i = threadIdx.x; i < n; i += MEL_NORM_THREADS)
+        x[i] = (float)((fmax((double)x[i] * MEL_LOG10_E, lo) + 4.0) * 0.25);
+}
+
+__global__ void __launch_bounds__(MEL_NORM_THREADS)
+mel_norm_kernel(MelNorm mn) {
+    if (mn.flags & CLX_MEL_NORM_WHISPER) mel_norm_whisper(mn);
+    else mel_norm_per_feature(mn);
+}
+
+namespace {
+cudaError_t launch_mel_norm(const MelNorm& mn, cudaStream_t stream, uint64_t* launches) {
+    if (!mn.flags) return cudaSuccess;
+    const uint64_t warps = MEL_NORM_THREADS / 32, segs = (uint64_t)mn.n * mn.C * mn.n_mels;
+    const uint32_t ctas = (mn.flags & CLX_MEL_NORM_WHISPER)
+                              ? mn.n * mn.C  // (rows < 2^31: the mel crop create's check)
+                              : (uint32_t)std::min<uint64_t>(MEL_NORM_MAX_CTAS, (segs + warps - 1) / warps);
+    mel_norm_kernel<<<std::max(ctas, 1u), MEL_NORM_THREADS, 0, stream>>>(mn);
+    (*launches)++;
+    return cudaGetLastError();
+}
+}  // namespace
+
 cudaError_t mel_init() {  // the most any batch uses, so that no batch lowers another's limit
     cudaError_t e = cudaFuncSetAttribute(mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MEL_SMEM);
     if (e == cudaSuccess)
@@ -256,21 +352,23 @@ cudaError_t mel_init() {  // the most any batch uses, so that no batch lowers an
     return e;
 }
 
-cudaError_t launch_mel(const MelBuffers& mb, size_t smem, cudaStream_t stream, uint64_t* launches) {
+cudaError_t launch_mel(const MelBuffers& mb, const MelNorm& mn, size_t smem, cudaStream_t stream, uint64_t* launches) {
     mel_kernel<<<mb.rows * mb.tiles, MEL_THREADS, smem, stream>>>(mb);
     (*launches)++;
-    return cudaGetLastError();
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? launch_mel_norm(mn, stream, launches) : e;
 }
 
-cudaError_t launch_mel_packed(const MelBuffers& mb, const MelPacked& mp, size_t smem, cudaStream_t stream,
-                              uint64_t* launches) {
+cudaError_t launch_mel_packed(const MelBuffers& mb, const MelPacked& mp, const MelNorm& mn, size_t smem,
+                              cudaStream_t stream, uint64_t* launches) {
     mel_packed_plan_kernel<<<1, SCAN_THREADS, 0, stream>>>(mp, mb.n_fft, mb.hop, (mb.flags & CLX_MEL_CENTER) != 0);
     (*launches)++;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     mel_packed_kernel<<<mb.rows * mb.tiles, MEL_THREADS, smem, stream>>>(mb, mp);
     (*launches)++;
-    return cudaGetLastError();
+    e = cudaGetLastError();
+    return e == cudaSuccess ? launch_mel_norm(mn, stream, launches) : e;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -287,8 +385,13 @@ bool smooth(uint32_t n) {  // no prime factor above 5
 bool mel_params_ok(const clx_mel_params* p) {
     if (!p) return false;
     const uint32_t n_fft = p->n_fft;
+    const uint32_t norm = p->flags & (CLX_MEL_NORM_PER_FEATURE | CLX_MEL_NORM_WHISPER);
     if (n_fft % 2 || n_fft < 8 || n_fft > 4096 || !smooth(n_fft / 2) || p->win_length < 1 || p->win_length > n_fft ||
-        p->hop_length < 1 || p->n_mels < 1 || p->n_mels > 512 || (p->flags & ~(CLX_MEL_CENTER | CLX_MEL_LOG)))
+        p->hop_length < 1 || p->n_mels < 1 || p->n_mels > 512 || (p->flags & ~(CLX_MEL_CENTER | CLX_MEL_LOG | norm)))
+        return false;
+    // a normalisation needs the log of centred frames, and takes one map
+    if (norm && (norm == (CLX_MEL_NORM_PER_FEATURE | CLX_MEL_NORM_WHISPER) ||
+                 (p->flags & (CLX_MEL_LOG | CLX_MEL_CENTER)) != (CLX_MEL_LOG | CLX_MEL_CENTER)))
         return false;
     return (p->flags & CLX_MEL_LOG) ? std::isfinite(p->log_floor) && p->log_floor > 0.f : p->log_floor == 0.f;
 }
@@ -350,6 +453,7 @@ size_t mel_packed_frames(const clx_mel_params* p, size_t max_excerpts, size_t ma
 }  // namespace clx
 
 extern "C" size_t clx_mel_packed_frames_bound(const clx_mel_params* params, size_t max_excerpts, size_t max_samples) {
-    if (!clx::mel_params_ok(params) || max_excerpts == 0 || max_samples == 0) return 0;
+    if (!clx::mel_params_ok(params) || (params->flags & CLX_MEL_NORM_WHISPER) || max_excerpts == 0 || max_samples == 0)
+        return 0;
     return clx::mel_packed_frames(params, max_excerpts, max_samples);
 }

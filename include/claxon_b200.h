@@ -543,9 +543,24 @@ size_t clx_resample_packed_source_bound(const uint32_t* file_rates, size_t n_fil
  * 4096 or with n_fft / 2 having a prime factor above 5; win_length 0 or above n_fft; hop_length 0; n_mels 0 or above
  * 512; other flags; with CLX_MEL_LOG a log_floor that is not finite and > 0, without it one that is not 0; a window or
  * fbank value that is not finite; num_frames <= n_fft / 2 with CLX_MEL_CENTER (torch.stft refuses that reflect pad),
- * num_frames < n_fft without; sizes that overflow. */
+ * num_frames < n_fft without; sizes that overflow.
+ * Normalised features: with CLX_MEL_NORM_PER_FEATURE or CLX_MEL_NORM_WHISPER (each needs CLX_MEL_LOG and
+ * CLX_MEL_CENTER; not both) one more kernel, mel_norm_kernel, rewrites the log features in place after the mel kernel,
+ * each reduction and map in float64 with one rounding to float32, in a fixed order without atomics.
+ * CLX_MEL_NORM_PER_FEATURE: for each (crop b, row, mel), x its first v_b frames with v_b = 1 + n_b / hop_length (n_b
+ * the crop's length in samples; v_b = 0 when n_b = 0), mu = mean(x), sigma = sqrt(sum (x - mu)^2 / (v_b - 1)) (0 when
+ * v_b = 1) and y = (x - mu) / (sigma + 1e-5): NeMo's per_feature normalize_batch with torch.stft's frame count.  Frames
+ * t >= v_b read exactly 0, so an invalid crop is all 0, and so are rows its file does not have (constant features).
+ * CLX_MEL_NORM_WHISPER: the output has F' = F - 1 frames (Whisper drops the last STFT frame; the kept frames are those
+ * of the unnormalised batch bit for bit) and, with l = x / ln 10 and M the largest l of the row's [n_mels, F'], y =
+ * (max(l, M - 8) + 4) / 4: WhisperFeatureExtractor's log-mel of the crop as its zero-padded input.  Refused when F < 2.
+ * Each call is then the inner batch's launch sequence and two kernels.  Also CLX_ERR_INVALID_ARGUMENT for a
+ * normalisation flag without both CLX_MEL_LOG and CLX_MEL_CENTER, for both flags, and for CLX_MEL_NORM_PER_FEATURE with
+ * n_crops * C * n_mels (max_excerpts * C * n_mels for packed batches) of 2^31 or more. */
 #define CLX_MEL_CENTER 1u  /* reflect-pad n_fft / 2 samples on each side (torch.stft center=True, pad_mode "reflect") */
 #define CLX_MEL_LOG 2u     /* store ln(max(mel, log_floor)) */
+#define CLX_MEL_NORM_PER_FEATURE 4u  /* per-(crop or excerpt, row, mel) mean / variance over the valid frames */
+#define CLX_MEL_NORM_WHISPER 8u      /* Whisper's clamp to the row's max - 8 in log10 and (l + 4) / 4; crops only */
 typedef struct clx_mel_params {
     uint32_t n_fft;       /* even, 8 .. 4096, n_fft / 2 with no prime factor above 5 (400, 512, 320, 480, 1024, 2048 ...) */
     uint32_t win_length;  /* 1 .. n_fft */
@@ -581,8 +596,11 @@ int clx_batch_create_mel_crops(clx_ctx* ctx, clx_corpus* corpus, const uint32_t*
  * n_mels * T_f floats, 16 bytes per excerpt and tables of a few times n_fft floats.
  * CLX_ERR_INVALID_ARGUMENT for what the inner create refuses; every parameter clx_batch_create_mel_crops refuses (NULL
  * params, window or fbank, n_fft, win_length, hop_length, n_mels, flags, log_floor, non-finite window or fbank values);
- * max_excerpts 0 or 2^30 or more, max_samples 0; sizes that overflow.  No length is refused: a too short excerpt has 0
- * frames. */
+ * max_excerpts 0 or 2^30 or more, max_samples 0; sizes that overflow; CLX_MEL_NORM_WHISPER (Whisper's input is a fixed
+ * window).  No length is refused: a too short excerpt has 0 frames.
+ * With CLX_MEL_NORM_PER_FEATURE, each (excerpt b, row c, mel m) of F_b > 0 frames is normalised over those F_b frames
+ * as clx_batch_create_mel_crops normalises a crop's valid frames; the layout, starts and frame counts do not change and
+ * every other element still reads 0.  Each call then runs a third kernel, one warp per (excerpt, row, mel). */
 int clx_batch_create_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t* file_rates, size_t n_files,
                                 size_t max_excerpts, size_t max_samples, uint32_t target_rate,
                                 const clx_mel_params* params, const float* window /* win_length */,
@@ -591,7 +609,8 @@ int clx_batch_create_mel_packed(clx_ctx* ctx, clx_corpus* corpus, const uint32_t
  * (T) columns of max_excerpts (B), a multiple of 4.  With m the shortest length that has a frame (n_fft / 2 + 1 with
  * CLX_MEL_CENTER, n_fft without) and k = min(B, (T - m) / round_up_4(m) + 1) the most excerpts with frames that fit:
  * round_up_4(floor(T / hop_length) + 4k), and 0 when T < m.  SIZE_MAX if that overflows.  0 also for params that
- * clx_batch_create_mel_crops refuses, or a zero argument.  Host only; no context. */
+ * clx_batch_create_mel_crops refuses, CLX_MEL_NORM_WHISPER, or a zero argument; CLX_MEL_NORM_PER_FEATURE does not
+ * change it.  Host only; no context. */
 size_t clx_mel_packed_frames_bound(const clx_mel_params* params, size_t max_excerpts, size_t max_samples);
 /* Device pointer of a mel packed batch's max_excerpts int64 frame counts F_b (NULL for other batches). */
 void* clx_batch_mel_frames(clx_batch* b);
